@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- sliding-window solves/sec on synthetic 10-frame x 150-feature windows (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 N > 1 is launched by torchrun (one rank per GPU); the windows are independent, so the batch is split across ranks
 with no data-path collective (weak scaling: 1024 windows per GPU) and NCCL is only used for the barrier and the
@@ -15,7 +15,10 @@ dogleg iterations) over one batch of 1024 windows per GPU.
           are + device pack + solve + D2H inside the timed region
   --impl reference : the CPU path (oracle port of the reference's Ceres solve; the reference itself cannot be
           compiled here) on all host cores over the same 1024-window batch per step.
-Inputs per step (about 340 MB per GPU) are larger than the 126 MB L2, so no explicit L2 flush is needed.
+Inputs per step (about 340 MB per GPU) are larger than the 50 MB L2 of an H100, so no explicit L2 flush is needed.
+--dump-outputs DIR : after the timed resident steps, rank 0 writes what the last step computed, as a caller of
+          cerb_batch_download receives it (solved states, inverse depths, solve reports), to DIR/<name>.npy.  The synthetic
+          inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -38,7 +41,7 @@ def static_config(NW, F, world):
     """The part of `config` that names the workload: identical on the GPU arm and the reference arm."""
     return {"workload": f"{NW} independent synthetic 10-frame x {F}-feature stereo windows per GPU (BASELINE.json configs[1]): {F * 21} visual factors, 10 IMU-leg factors, dense 86-dim marginalization prior, extrinsics free, <= 12 dogleg iterations (all 12 are used)",
             "windows_per_gpu": NW, "features": F,
-            "l2": "inputs per step (~300 MB/GPU) exceed the 126 MB L2; no explicit flush",
+            "l2": "inputs per step (~300 MB/GPU) exceed the 50 MB L2; no explicit flush",
             "parallelism": f"batch split x{world}, no data-path collective"}
 
 
@@ -176,6 +179,20 @@ def emit(line):
     os.write(_REAL_STDOUT if _REAL_STDOUT is not None else 1, (json.dumps(line) + "\n").encode())
 
 
+def dump_outputs(out_dir, gpu, batch):
+    """The results of the last resident solve as the caller receives them (float64; about 3.4 MB at the default size)."""
+    import numpy as np
+    rep = gpu.download(batch)
+    st = batch.state_array()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {name: st[name] for name in ("para_Pose", "para_SpeedBias", "para_LegBias", "para_Ex_Pose", "para_Td")}
+    arrays["para_Feature"] = batch.para_Feature
+    for name in ("iterations", "num_successful_steps", "termination", "initial_cost", "final_cost"):
+        arrays["report_" + name] = rep[name]
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
 def main():
     _quiet_stdout()
     ap = argparse.ArgumentParser()
@@ -187,6 +204,7 @@ def main():
     ap.add_argument("--features", type=int, default=FEATURES)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--distinct", type=int, default=0, help="distinct synthetic windows to generate (tiled up to --windows); 0: all distinct up to 200 features, else 64")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the last timed step to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -240,6 +258,8 @@ def main():
             ms, nl = gpu.last_solve_stats()
             ev_ms += ms; launches += nl
         wall_resident = time.perf_counter() - t0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, gpu, batch)
         barrier()
         # ---- end to end through the host-buffer call ---------------------------------------------------------------
         e2e_s = 0.0
@@ -272,20 +292,9 @@ def main():
     d2h = int(NW * (240 * 8 + cfg.max_features * 8 + C.sizeof(abi.SolveReport)))
 
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = 3350.0
+        peak_src = "H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s), not a measured peak"
         traffic = None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "solve_kernel_traffic.json")))
-            if tj.get("windows") == NW and tj.get("features") == F:       # the ncu capture is of the default workload only
-                traffic = tj.get("dram_bytes_per_launch")
-        except Exception:
-            pass
         kernel_s = ev_ms * 1e-3 / args.steps
         achieved = b_alg(F) * NW / kernel_s / 1e9
         line = {

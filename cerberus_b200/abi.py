@@ -1,4 +1,4 @@
-"""ctypes mirror of include/cerberus_b200.h (the C ABI of the B200 VILO backend).
+"""ctypes mirror of include/cerberus_b200.h (the C ABI of the H100 VILO backend).
 
 Pure declarations: struct layouts, enums and a `WindowBatch` container that owns contiguous numpy
 storage for a batch of sliding windows and exposes it as arrays of CerbWindowDesc /

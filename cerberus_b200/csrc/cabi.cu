@@ -1,4 +1,4 @@
-// cabi.cu -- implementation of the C ABI of include/cerberus_b200.h on top of the sm_100a kernels.
+// cabi.cu -- implementation of the C ABI of include/cerberus_b200.h on top of the sm_90a kernels.
 // Host side only packs the reference-shaped descriptors (AoS, Eigen column-major) into the device
 // layout (planar observations, compact preintegration records), moves them through pinned staging
 // buffers on the handle's stream and launches kernels.  There is no CPU compute path: if no CUDA
@@ -82,7 +82,7 @@ const char *cerb_version(void) {
 #if defined(CERB_CUSIM)
     return "cerberus_b200 0.1 (cusim test build)";
 #else
-    return "cerberus_b200 0.1 (sm_100a)";
+    return "cerberus_b200 0.1 (sm_90a)";
 #endif
 }
 
@@ -166,11 +166,10 @@ static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDev
     h->nfeat.assign(B, 0); h->n0.assign(B, 0);
     CUDA_TRY(cudaMemcpy(h->d_G, cfg->g, 3 * sizeof(double), cudaMemcpyHostToDevice));
 #if !defined(CERB_CUSIM)
-    // The per-CTA workspace (W, the prior Hessian image: ~290 KB x 148 CTAs) is re-read every iteration while ~300 KB of inputs per window
-    // stream through once per linearisation; a persisting access-policy window on the compute stream keeps the workspace in L2.  Measured
-    // on the B200 (profiles/README.md): DRAM traffic of the solve 7.8 x -> 6.3 x the algorithmic bytes, but the step gets 1.7 % SLOWER
-    // (23.08 ms vs 22.70 ms per 1024 windows, alternating runs on one box): DRAM is at < 1 % utilisation, the carve-out only takes L2 away
-    // from the inputs.  Hence opt-in (CERB_L2_PERSIST=1), off by default.
+    // The per-CTA workspace (W, the prior Hessian image: ~290 KB x one CTA per SM) is re-read every iteration while ~300 KB of inputs per
+    // window stream through once per linearisation; a persisting access-policy window on the compute stream can keep the workspace in L2.
+    // The solve is fp64-latency bound with DRAM nearly idle, so the carve-out mostly takes L2 away from the inputs: opt-in
+    // (CERB_L2_PERSIST=1), off by default.
     {
         const size_t ws_bytes = (size_t)h->grid * h->ws_stride * sizeof(double);
         const size_t want = std::min<size_t>(ws_bytes, (size_t)prop.persistingL2CacheMaxSize);

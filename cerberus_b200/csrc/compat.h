@@ -1,5 +1,5 @@
 // compat.h -- the handful of launch / qualifier macros the kernels are written against.
-// Product build (nvcc, sm_100a): plain CUDA.  With -DCERB_CUSIM (tests/cusim, g++) the same kernel
+// Product build (nvcc, sm_90a): plain CUDA.  With -DCERB_CUSIM (tests/cusim, g++) the same kernel
 // sources run on CPU threads so the non-GPU test tier can exercise the real kernel logic; that build
 // is test infrastructure, is never linked into libcerberus_b200.so and is never a fallback.
 #pragma once

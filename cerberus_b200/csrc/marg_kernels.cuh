@@ -28,7 +28,7 @@ constexpr int MARG_MAX_SWEEPS = 60;
 //            itself is never formed:  Arm Amm_inv [Amr | bm] = T^T diag(lambda > eps ? 1 / lambda : 0) T.  Columns [0, ncs) of T live in
 //            shared memory behind M1, the remaining ncg = n + 1 - ncs columns (0 for m <= ~165; 3 at m = 169) in the global workspace (L2)
 //   phase 2  M2 (n x n packed) over the dead M1, V2 (n x n) behind it over the dead T
-constexpr size_t MARG_SMEM_MAX = 232448;               // 227 KB: the opt-in limit of dynamic shared memory per block on sm_100 (the kernel has no static shared memory)
+constexpr size_t MARG_SMEM_MAX = 232448;               // 227 KB: the opt-in limit of dynamic shared memory per block on sm_90 (the kernel has no static shared memory)
 constexpr size_t MARG_SMEM_TWO = 115712;               // 113 KB: two CTAs of 256 threads per SM below this
 constexpr int MARG_N_STRUCT = 86;                      // kept dimension of a VILO window: 10 poses + speed-bias + leg bias + 2 extrinsics + td (SURVEY 8(a) a12)
 CERB_HD int marg_ld(int k) { return k | 1; }

@@ -1,4 +1,4 @@
-// vmath.cuh -- fp64 3-vector / 3x3 / quaternion helpers for the sm_100a kernels.
+// vmath.cuh -- fp64 3-vector / 3x3 / quaternion helpers for the sm_90a kernels.
 // Everything is __host__ __device__ so the same source also builds in the CPU kernel simulator used
 // by the non-GPU tests (tests/cusim); the shipped library only ever instantiates the device side.
 #pragma once

@@ -1,6 +1,6 @@
 """ctypes binding of libcerberus_b200.so (the C ABI of include/cerberus_b200.h).
 
-The product library is the nvcc-built sm_100a one next to this file; it has no CPU fallback and
+The product library is the nvcc-built sm_90a one next to this file; it has no CPU fallback and
 `Backend()` raises if it (or a CUDA device) is missing.  Tests that run without a GPU pass the path of
 the CPU kernel *simulator* build (tests/cusim) explicitly -- that is test infrastructure, never a default.
 """

@@ -1,8 +1,8 @@
 """Generate the frozen known-answer vectors of tests/golden/*.npz with the CPU oracle.
 
 The reference ships no golden vectors for this path.  The factor-level vectors (A1 kinematics, the three projection
-factors, the IMU-leg factor incl. sqrt_info) are outputs of THE REFERENCE'S OWN SOURCES, compiled where they lie under
-/root/reference/src against the header shims of oracle/shim (oracle/_ref/libcerberus_ref.so, `make -C oracle ref`).
+factors, the IMU-leg factor incl. sqrt_info) are outputs of THE REFERENCE'S OWN SOURCES, compiled where they lie against
+the header shims of oracle/shim (oracle/_ref/libcerberus_ref.so, `make -C oracle ref REF=<Cerberus checkout>/src`).
 The window-level vector (a full 12-iteration solve) comes from the oracle's restatement of ceres-solver 1.14, which is
 not available here.  Seeds of the inputs: the kinematics probe of src/test/ceres_test.cpp:16-18, the A1 geometry of
 estimator.cpp:143-156, the perturbation of imu_leg_factor.cpp:43.  Re-run:  python tests/golden/make_golden.py
@@ -29,7 +29,7 @@ def window_arrays(batch, w=0):
 
 def main():
     ob = OracleBackend()
-    ref = RefBackend()                  # the compiled reference sources generate the factor-level vectors
+    ref = RefBackend(live=True)         # the compiled reference sources generate the factor-level vectors
     out = {}
     # --- A1 kinematics at the probe of src/test/ceres_test.cpp:16-18, all four legs
     q = np.tile(np.array([0.1, 0.1, 0.3]), (4, 1))

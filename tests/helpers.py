@@ -87,3 +87,15 @@ def check_against_golden(backend, g, tol_scale=1.0, solve=True):
         assert np.abs(st["para_Ex_Pose"][0] - g["win_solved_ex"]).max() < 1e-7
         nf = g["win_solved_feature"].shape[0]
         assert np.abs(b.para_Feature[0][:nf] - g["win_solved_feature"]).max() < 1e-7
+
+
+SEAM = os.path.join(ROOT, "tests", "seam")
+
+
+def seam_probe(include_dir, workdir):
+    """The JSON printed by tests/seam/probe.cpp built against `include_dir` (tests/seam or the reference's src directory)."""
+    import json
+    exe = os.path.join(workdir, "seam_probe")
+    subprocess.run(["g++", "-std=c++14", "-w", "-I" + os.path.join(ROOT, "include"), "-I" + os.path.join(ROOT, "oracle", "shim"), "-I" + include_dir,
+                    os.path.join(SEAM, "probe.cpp"), "-o", exe], check=True, capture_output=True, text=True)
+    return json.loads(subprocess.run([exe], check=True, capture_output=True, text=True).stdout)

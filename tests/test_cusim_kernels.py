@@ -1,4 +1,4 @@
-"""The sm_100a kernel sources, run on CPU threads by tests/cusim, against the CPU oracle (non-GPU tier).
+"""The sm_90a kernel sources, run on CPU threads by tests/cusim, against the CPU oracle (non-GPU tier).
 The same comparisons run on the real device in test_gpu_parity.py."""
 import numpy as np
 import pytest
@@ -231,7 +231,7 @@ def _chained_windows_case(make_backend, nw=1, F=12, F0=8, iters=3, nthreads=4):
     out = []
     # Same eigen algorithm on both arms (cyclic Jacobi, the device's): this test pins the device chain against the restatement of the
     # SAME arithmetic.  What the choice of eigen-solver (the reference's tridiagonal QR vs Jacobi) does to a chained trajectory is
-    # measured over >= 20 frames by tools/eig_study.py / tests/test_replay.py (profiles/eig_study_r2.txt): the published poses move by
+    # measured over >= 20 frames by tools/eig_study.py / tests/test_replay.py: the published poses move by
     # 1e-4 .. 4e-4 m under ANY rounding-level change of the marginalization, including two QR runs that only differ in summation order.
     o.set_eig_mode(1)
     try:

@@ -1,7 +1,7 @@
 """Per-feature steps either side of the solve (SURVEY.md 8(f) n3): Estimator::outliersRejection and FeatureManager::triangulate
 on the resident batch.  CPU tier: the kernels on the CPU simulator vs the oracle restatement (estimator.cpp:1729-1798,
 feature_manager.cpp:198-212,302-385), the oracle's 4x4 null vector vs numpy's LAPACK SVD, and the geometry itself (a noise-free
-track triangulates to its true depth).  GPU tier: the sm_100a kernels vs the oracle."""
+track triangulates to its true depth).  GPU tier: the sm_90a kernels vs the oracle."""
 import numpy as np
 import pytest
 from cerberus_b200 import abi, synth

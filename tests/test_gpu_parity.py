@@ -1,4 +1,4 @@
-"""Parity of the sm_100a path against the CPU oracle on a real B200, through the C ABI (pytest -m gpu).
+"""Parity of the sm_90a path against the CPU oracle on a real H100, through the C ABI (pytest -m gpu).
 
 Bar (BASELINE.json north_star): per-window pose delta < 1e-4 m against the reference-semantics CPU solve; measured
 deltas are ~1e-9 m, the assertions use 1e-6 m.  Full-size cases (1024 windows) are checked through size-independent
@@ -189,7 +189,7 @@ def test_chained_windows_match_oracle_gpu():
 
 
 def test_edge_windows_gpu():
-    """A window without visual factors, a window with a single feature (12 iterations on the sm_100a build)."""
+    """A window without visual factors, a window with a single feature (12 iterations on the sm_90a build)."""
     from test_cusim_kernels import _empty_and_single_feature_case
     _empty_and_single_feature_case(lambda cfg: lib.Backend(cfg), iters=12)
 

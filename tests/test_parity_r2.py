@@ -7,19 +7,19 @@ CPU tier (`-m "not gpu"`):
   * the per-feature steps (triangulate / outlier errors / depth shift) of the oracle and of the kernels (CPU simulator) against
     the reference's own FeatureManager (featureTracker/feature_manager.cpp compiled into oracle/_ref) and the statements of
     Estimator::reprojectionError / outliersRejection executed over it.
-GPU tier (`-m gpu`): the sm_100a build of cerb_preintegrate_imu_batch, cerb_eval_imu, cerb_eval_prior, the sum_dt > 10 skipped
+The reference arm replays the stored outputs of those sources (tests/golden/ref_v1.npz, see tests/oracle_lib.py).
+GPU tier (`-m gpu`): the sm_90a build of cerb_preintegrate_imu_batch, cerb_eval_imu, cerb_eval_prior, the sum_dt > 10 skipped
 factor, MARGIN_SECOND_NEW and marginalization with an old prior, the per-feature steps against the reference sources."""
 import ctypes as C
 import os
 import numpy as np
 import pytest
 from cerberus_b200 import abi, synth, lib
-from oracle_lib import OracleBackend, RefBackend, ref_lib
+from oracle_lib import OracleBackend, RefBackend, ref_rows, sub_jobs
 from helpers import sim_backend, small_cfg, prior_canonical, state_diffs, SIM_LIB
 from test_preintegration import make_jobs
 
 ob = OracleBackend()
-needs_ref = pytest.mark.skipif(ref_lib() is None, reason="oracle/_ref not built and /root/reference absent")
 
 
 # ---------------------------------------------------------------------------------------------------- double2vector
@@ -60,12 +60,12 @@ D2V_PITCHES = [(5.0, -7.0), (30.0, 29.0), (-45.0, -44.0), (89.6, 20.0), (10.0, -
 
 def _check_d2v(cdll):
     rng = np.random.default_rng(12)
-    ref = RefBackend() if ref_lib() is not None else None
+    ref = RefBackend()
     singular = 0
-    for (pb, pa) in D2V_PITCHES * 3:
+    for k, (pb, pa) in enumerate(D2V_PITCHES * 3):
         before, after = _d2v_states(rng, pb, pa)
         got = _d2v_product(cdll, before, after)
-        for arm in ([ob] if ref is None else [ob, ref]):
+        for arm in ((ob, ref) if k < len(D2V_PITCHES) else (ob,)):      # the reference arm on the first pass over the pitches
             want = arm.double2vector(before, after)
             for g, w, name in zip(got, want, ("Ps", "Rs", "Vs")):
                 assert np.abs(g - w).max() < 1e-12 * max(1.0, np.abs(w).max()), (name, pb, pa, type(arm).__name__)
@@ -78,14 +78,12 @@ def _check_d2v(cdll):
     assert singular >= 9
 
 
-@needs_ref
 def test_double2vector_sim_build_vs_oracle_and_reference():
     _check_d2v(C.CDLL(SIM_LIB) if os.path.exists(SIM_LIB) else sim_backend(small_cfg()).lib)
 
 
-@needs_ref
 def test_double2vector_product_library_vs_oracle_and_reference():
-    """The sm_100a library's host-side cerb_double2vector (no device involved: callable without a GPU)."""
+    """The sm_90a library's host-side cerb_double2vector (no device involved: callable without a GPU)."""
     if not os.path.exists(lib.PRODUCT_LIB):
         pytest.skip("product library not built")
     try:
@@ -96,24 +94,40 @@ def test_double2vector_product_library_vs_oracle_and_reference():
 
 
 # ---------------------------------------------------------------------------------------------------- n3 against reference source
-@needs_ref
 @pytest.mark.parametrize("realistic", [False, True])
 def test_feature_steps_oracle_and_sim_vs_reference_feature_manager(realistic):
     """FeatureManager::{triangulate, triangulatePoint, removeBackShiftDepth} (feature_manager.cpp:198-212,302-385,450-488) and the
-    statements of Estimator::{reprojectionError, outliersRejection} (estimator.cpp:1729-1798) executed from the reference's source."""
-    from test_feature_steps import _check_backend, _batch
+    statements of Estimator::{reprojectionError, outliersRejection} (estimator.cpp:1729-1798) executed from the reference's source,
+    against the oracle restatement and the kernels (CPU simulator).  The kernels along a solve are checked against the oracle by
+    test_feature_steps.py."""
     cfg = small_cfg(max_batch=4, max_features=24, iters=3)
+    _check_feature_steps_vs_reference(ob, realistic)
+    _check_feature_steps_vs_reference(sim_backend(cfg), realistic)
+
+
+def _feature_steps(arm, batch):
+    """(outlier errors, triangulated depths, (start frame, depth, keep) of the depth shift) of `arm` at the batch's states: the
+    oracle and the reference read the host batch, a library backend gets it uploaded before each step."""
+    if not isinstance(arm, lib.Backend):
+        return arm.outlier_errors(batch), arm.triangulate(batch), arm.shift_depth(batch, 6.5)
+    arm.upload(batch); e = arm.outlier_errors(batch.n)[0]
+    arm.upload(batch); t = arm.triangulate(batch.n)
+    arm.upload(batch); s = arm.shift_depth(batch.n, 6.5)
+    return e, t, s
+
+
+def _check_feature_steps_vs_reference(arm, realistic):
+    """The per-feature steps of `arm` against the reference's FeatureManager on the windows of test_feature_steps._batch (built by the
+    oracle, so the inputs do not depend on the arm), once as generated and once with every second track not triangulated."""
+    from test_feature_steps import _batch
     ref = RefBackend()
-    # oracle restatement vs reference source
     batch = _batch(ob, realistic)
     nf = [batch.descs[w].n_features for w in range(batch.n)]
     for lamset in (0, 1):
         if lamset:
             for w in range(batch.n):
                 batch.para_Feature[w, 0:nf[w]:2] = -1.0
-        e0, e1 = ob.outlier_errors(batch), ref.outlier_errors(batch)
-        t0, t1 = ob.triangulate(batch), ref.triangulate(batch)
-        s0, s1 = ob.shift_depth(batch, 6.5), ref.shift_depth(batch, 6.5)
+        (e0, t0, s0), (e1, t1, s1) = _feature_steps(arm, batch), _feature_steps(ref, batch)
         for w in range(batch.n):
             k = nf[w]
             if not lamset:
@@ -123,8 +137,6 @@ def test_feature_steps_oracle_and_sim_vs_reference_feature_manager(realistic):
             keep = s1[2][w, :k] != 0
             assert (s0[0][w, :k][keep] == s1[0][w, :k][keep]).all() and (s0[2][w, :k] == s1[2][w, :k]).all()
             assert np.abs(s0[1][w, :k][keep] - s1[1][w, :k][keep]).max() < 1e-12 * np.abs(s1[1][w, :k][keep]).max()
-    # kernels (CPU simulator) vs reference source
-    _check_backend(sim_backend(cfg), ref, realistic)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU tier
@@ -134,29 +146,28 @@ def _gpu(cfg=None):
 
 @pytest.mark.gpu
 def test_double2vector_product_library_gpu_box():
-    ref_ok = ref_lib() is not None
-    assert ref_ok, "oracle/_ref/libcerberus_ref.so travels with the snapshot"
     _check_d2v(_gpu().lib)
 
 
 @pytest.mark.gpu
 def test_imu_preintegration_and_imu_factor_gpu():
-    """Row a9 / a6 on the sm_100a build: cerb_preintegrate_imu_batch and cerb_eval_imu vs the oracle and the reference's
+    """Row a9 / a6 on the sm_90a build: cerb_preintegrate_imu_batch and cerb_eval_imu vs the oracle and the reference's
     integration_base.h / imu_factor.h (oracle/_ref)."""
     from test_reference_pin import imu_setup
     gpu = _gpu()
-    arms = [ob] + ([RefBackend()] if ref_lib() is not None else [])
+    ref = RefBackend()
     jobs, _, _ = make_jobs(6, seed=29)
     pcfg = abi.default_preint_config()
     got = gpu.preintegrate_imu(pcfg, jobs, 6)
-    for arm in arms:
-        want = arm.preintegrate_imu(pcfg, jobs, 6)
+    rows = ref_rows(6, 2)
+    for arm, want, sel in ((ob, ob.preintegrate_imu(pcfg, jobs, 6), slice(None)), (ref, ref.preintegrate_imu(pcfg, sub_jobs(jobs, rows), len(rows)), rows)):
         for name in want.dtype.names:
-            assert np.abs(got[name] - want[name]).max() <= 1e-11 * max(1e-30, np.abs(want[name]).max()), (name, type(arm).__name__)
+            assert np.abs(got[sel][name] - want[name]).max() <= 1e-11 * max(1e-30, np.abs(want[name]).max()), (name, type(arm).__name__)
     pre, params = imu_setup(4)
-    r1, j1, s1 = gpu.eval_imu(pre, params)
-    for arm in arms:
-        r0, j0, s0 = arm.eval_imu(pre, params)
+    rows = ref_rows(4, 1)
+    out = gpu.eval_imu(pre, params)
+    for arm, (r0, j0, s0), sel in ((ob, ob.eval_imu(pre, params), slice(None)), (ref, ref.eval_imu(pre[rows], params[rows]), rows)):
+        r1, j1, s1 = (x[sel] for x in out)
         assert np.abs(s0 - s1).max() < 1e-9 * np.abs(s0).max() and np.abs(r0 - r1).max() < 1e-9 * np.abs(r0).max() and np.abs(j0 - j1).max() < 1e-9 * np.abs(j0).max()
     # the windows a USE_LEG == 0 estimator would solve, fed by the DEVICE preintegration on one arm and the oracle's on the other
     cfg = small_cfg(max_batch=4, max_features=32)
@@ -182,14 +193,16 @@ def test_prior_evaluator_gpu():
     pr = batch.descs[0].prior
     ncols = 7 * 12 + 9 + 4 + 1
     r1, j1 = gpu.eval_prior(pr, batch.states[0], ncols)
-    for arm in [ob] + ([RefBackend()] if ref_lib() is not None else []):
-        r0, j0 = arm.eval_prior(pr, batch.states[0], ncols)
-        assert np.abs(r0 - r1).max() < 1e-10 * np.abs(r0).max() and np.abs(j0 - j1).max() == 0.0
+    rows = ref_rows(pr.n, 12)
+    r2, j2 = ob.eval_prior(pr, batch.states[0], ncols)
+    for (r0, j0), sel in (((r2, j2.reshape(pr.n, ncols)), slice(None)), (RefBackend().eval_prior(pr, batch.states[0], ncols, rows), rows)):
+        r1s, j1s = r1[sel], j1.reshape(pr.n, ncols)[sel]
+        assert np.abs(r0 - r1s).max() < 1e-10 * np.abs(r0).max() and np.abs(j0 - j1s).max() == 0.0
 
 
 @pytest.mark.gpu
 def test_skipped_imu_factor_gpu():
-    """estimator.cpp:1119 (sum_dt > 10: factor not added) on the sm_100a build."""
+    """estimator.cpp:1119 (sum_dt > 10: factor not added) on the sm_90a build."""
     cfg = small_cfg(max_batch=4, max_features=32, iters=6)
     o, g = OracleBackend(cfg), lib.Backend(cfg)
     batch = synth.generate_batch(3, 24, o, window0=31, prior_features=8)
@@ -208,17 +221,16 @@ def test_skipped_imu_factor_gpu():
 @pytest.mark.gpu
 @pytest.mark.parametrize("margin_old", [True, False])
 def test_marginalization_with_prior_gpu(margin_old):
-    """MARGIN_OLD with an existing prior and MARGIN_SECOND_NEW on the sm_100a build vs the reference's MarginalizationInfo classes and the oracle."""
+    """MARGIN_OLD with an existing prior and MARGIN_SECOND_NEW on the sm_90a build vs the reference's MarginalizationInfo classes and the oracle."""
     cfg = small_cfg()
     gpu = lib.Backend(cfg)
     mk = lambda: synth.generate_batch(2, 10, ob, with_prior=True, window0=47)
     src = mk()
-    arms = [ob] + ([RefBackend()] if ref_lib() is not None else [])
     c = mk(); gpu.marginalize(cfg, src, c, margin_old)
-    for arm in arms:
-        a = mk(); arm.marginalize(cfg, src, a, margin_old)
-        for w in range(2):
-            A0, b0, x0 = prior_canonical(a, w); A1, b1, x1 = prior_canonical(c, w)
+    a = mk(); ob.marginalize(cfg, src, a, margin_old)
+    for want in ([prior_canonical(a, w) for w in range(2)], RefBackend().marginal_priors(cfg, synth.tile_batch(src, 1), margin_old)):
+        for w in range(len(want)):
+            (A0, b0, x0), (A1, b1, x1) = want[w], prior_canonical(c, w)
             assert A0.shape[0] == (86 if margin_old else 80) and A0.shape == A1.shape and set(x0) == set(x1)
             assert np.abs(A0 - A1).max() < 1e-5 * np.abs(A0).max() and np.abs(b0 - b1).max() < 1e-4 * np.abs(b0).max()
             assert all(np.abs(x0[k][:7] - x1[k][:7]).max() == 0 for k in x0)
@@ -227,10 +239,7 @@ def test_marginalization_with_prior_gpu(margin_old):
 @pytest.mark.gpu
 @pytest.mark.parametrize("realistic", [False, True])
 def test_feature_steps_gpu_vs_reference_feature_manager(realistic):
-    from test_feature_steps import _check_backend
-    assert ref_lib() is not None
-    cfg = small_cfg(max_batch=4, max_features=24, iters=4)
-    _check_backend(lib.Backend(cfg), RefBackend(), realistic)
+    _check_feature_steps_vs_reference(lib.Backend(small_cfg(max_batch=4, max_features=24, iters=4)), realistic)
 
 
 @pytest.mark.gpu

@@ -5,7 +5,7 @@ through cerberus_b200.estimator (the host mirror of Estimator / FeatureManager);
 The same driver runs on the CPU oracle (tests/oracle_lib.OracleOps) -- the reference arm -- and the published pose of every frame is
 compared.  Eigen-solver of the oracle arm = cyclic Jacobi like the device (identical arithmetic => tight tolerance); the distance to the
 tridiagonal-QR arm (the reference's kind of solver) is reported and bounded by the measured sensitivity of the chain
-(profiles/eig_study_r2.txt: 1e-4 .. 1e-3 m between ANY two rounding-different marginalizations)."""
+(tools/eig_study.py: 1e-4 .. 1e-3 m between ANY two rounding-different marginalizations)."""
 import os
 import time
 import numpy as np
@@ -55,7 +55,7 @@ def test_replay_matches_oracle_sim(tmp_path):
 
 @pytest.mark.gpu
 def test_replay_50_frames_gpu():
-    """GPU tier: 4 robots x 62 frames = 52 chained optimization() calls each through the sm_100a library."""
+    """GPU tier: 4 robots x 62 frames = 52 chained optimization() calls each through the sm_90a library."""
     n, n_frames = 4, 62
     seq, dev, arms, t_dev = _replay(lambda cfg: lib.Backend(cfg), n, n_frames, 90, 160, 12, eig_modes=(1, 0))
     steps = n_frames - 10
@@ -64,7 +64,7 @@ def test_replay_50_frames_gpu():
     P, _ = dev.poses()
     err = np.linalg.norm(P - seq.p[:, 10:10 + P.shape[1]], axis=-1)
     T = dev.timing
-    lines = [f"replay: {n} robots x {steps} frames through cerberus_b200 (sm_100a), wall {t_dev:.2f} s = {n * steps / t_dev:.1f} frames/s "
+    lines = [f"replay: {n} robots x {steps} frames through cerberus_b200 (sm_90a), wall {t_dev:.2f} s = {n * steps / t_dev:.1f} frames/s "
              f"(host mirror is Python; device + ABI time: solve {T['solve']:.2f} s, marginalize {T['marginalize']:.2f} s, preintegrate {T['preintegrate']:.2f} s, "
              f"triangulate {T['triangulate']:.2f} s, outliers {T['outliers']:.2f} s, shift {T['shift']:.2f} s, host bookkeeping {T['host']:.2f} s)",
              "per-frame max |published position delta| device vs oracle (same Jacobi eigen arithmetic) [m]: " + " ".join(f"{v:.1e}" for v in dP),
@@ -79,7 +79,7 @@ def test_replay_50_frames_gpu():
     # One optimization() on identical inputs agrees to ~1e-9 m (tests/test_gpu_parity.py); along a chain every arm re-linearises on its own
     # states, and the eps-clamped eigen factoring of the marginalization amplifies rounding-level differences: the first frames stay at
     # solve-level agreement, later ones wander inside the chain's measured sensitivity band (1e-4 .. 1.3e-3 m between ANY two
-    # rounding-different arms over 40 frames, also two QR arms: profiles/eig_study_r2.txt; measured here on the B200: 3.7e-4 m max against
+    # rounding-different arms over 40 frames, also two QR arms: tools/eig_study.py; measured on the GPU: 3.7e-4 m max against
     # the Jacobi arm, 3.7e-4 m against the QR arm over 52 frames) -- three orders of magnitude below the 3 .. 9 cm distance of every arm from the truth.
     assert dP[:3].max() < 1e-5 and dR[:3].max() < 1e-5, (dP[:3], dR[:3])
     assert dP.max() < 2e-3 and dR.max() < 2e-3, (dP.max(), dR.max())
@@ -110,7 +110,7 @@ def test_native_replay_matches_python_mirror_sim():
 
 @pytest.mark.gpu
 def test_native_replay_gpu():
-    """C++ host mirror on the B200: (1) 4 robots x 52 frames against the Python mirror over the same library and against the oracle arm;
+    """C++ host mirror on the GPU: (1) 4 robots x 52 frames against the Python mirror over the same library and against the oracle arm;
     (2) 256 robots x 20 frames: the batched replay the Python mirror cannot keep up with (8 ms of bookkeeping per robot and frame)."""
     n, n_frames, F = 4, 62, 160
     cfg = abi.default_config(); cfg.max_batch = n; cfg.max_features = 2 * F; cfg.max_obs = 2 * F * 11

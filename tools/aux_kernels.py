@@ -1,5 +1,5 @@
 """Drives every kernel outside the timed solve step once at benchmark scale, so that one ncu metric pass gives their
-duration and DRAM traffic (profiles/aux_kernels_*.csv):
+duration and DRAM traffic:
 
     ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none \
         -k regex:'preintegrate|marg|outlier|triangulate|shift_depth|projection_eval|imu_leg_eval|prior_eval' --csv \

@@ -26,8 +26,8 @@ pcfg = abi.default_preint_config()
 seq = synth.generate_sequence(n, nf, tracked=tracked, max_len=16, min_len=3)
 arms = {"A oracle/QR": oracle_lib.OracleOps(cfg, eig_mode=0), "B oracle/Jacobi": oracle_lib.OracleOps(cfg, eig_mode=1)}
 if oracle_lib.ref_lib() is not None:
-    arms["C reference classes/QR"] = oracle_lib.OracleOps(cfg, eig_mode=0, marg=oracle_lib.RefBackend())
-    arms["D reference classes/Jacobi"] = oracle_lib.OracleOps(cfg, eig_mode=1, marg=oracle_lib.RefBackend())
+    arms["C reference classes/QR"] = oracle_lib.OracleOps(cfg, eig_mode=0, marg=oracle_lib.RefBackend(live=True))
+    arms["D reference classes/Jacobi"] = oracle_lib.OracleOps(cfg, eig_mode=1, marg=oracle_lib.RefBackend(live=True))
 runs = {}
 for name, ops in arms.items():
     d = estimator.ReplayDriver(ops, cfg, pcfg, n, max_features=256).run(seq)

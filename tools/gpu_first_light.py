@@ -1,4 +1,4 @@
-"""First-light check on a real B200: parity of the GPU solve vs the CPU oracle + a first timing."""
+"""First-light check on a real H100: parity of the GPU solve vs the CPU oracle + a first timing."""
 import sys, time, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))

@@ -1,10 +1,11 @@
 // tools/integration_stub.cpp -- the reference-side binding of INTEGRATION.md as compilable C++ (C++14, like the reference).
-// It is compiled (syntax + types only) by tests/test_abi.py against include/cerberus_b200.h, the reference's own headers where they lie
-// (/root/reference/src: feature_manager.h, imu_leg_integration_base.h, marginalization_factor.h, parameters.h) and the header shims of
-// oracle/shim that stand in for Eigen / Ceres / ROS / OpenCV:
-//     g++ -std=c++14 -fsyntax-only -Iinclude -Ioracle/shim -I/root/reference/src tools/integration_stub.cpp
+// tests/test_abi.py compiles it (syntax + types only) against include/cerberus_b200.h, the header shims of oracle/shim that stand in
+// for Eigen / Ceres / ROS / OpenCV, and the reference's interface it reads: tests/seam declares those members (pinned to the
+// reference's feature_manager.h, imu_leg_integration_base.h, marginalization_factor.h and parameters.h by tests/golden/seam_v1.json);
+// with a Cerberus checkout the reference's own headers can be used instead:
+//     g++ -std=c++14 -fsyntax-only -Iinclude -Ioracle/shim -I$CERBERUS_SRC tools/integration_stub.cpp
 // `EstimatorSeam` lists the members of class Estimator (src/estimator/estimator.h:134-241) that optimization() touches at the seam;
-// estimator.h itself drags in the ROS node, the feature tracker and OpenCV and cannot be compiled here.
+// estimator.h itself drags in the ROS node, the feature tracker and OpenCV.
 #include <cstring>
 #include <vector>
 #include "cerberus_b200.h"

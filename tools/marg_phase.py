@@ -5,7 +5,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 from cerberus_b200 import abi, lib
-NW = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+NW = int(sys.argv[1]) if len(sys.argv) > 1 else 132
 NAMES = {46: "T stage loads (thread 0)", 40: "X: 2x2 blocks (thread 0)", 41: "barrier 1 (thread 0)", 42: "Y: V / T rotations (thread 0)", 43: "barrier 2 (thread 0)",
          47: "angle thread: X + barrier 1", 44: "angle thread: angles", 45: "angle thread: barrier 2"}
 cfg = abi.default_config(); cfg.max_batch, cfg.max_features, cfg.max_obs = 2, 8, 88

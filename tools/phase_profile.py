@@ -5,7 +5,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 from cerberus_b200 import abi, synth, lib
-NW = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+NW = int(sys.argv[1]) if len(sys.argv) > 1 else 132
 F = int(sys.argv[2]) if len(sys.argv) > 2 else 150
 REP = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 NAMES = {0: "zero+geometry", 1: "vision_linearize (total)", 2: "inertial_linearize (total)", 3: "post-linearize (sums, symmetrise, scaling)",

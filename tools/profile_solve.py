@@ -4,7 +4,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 from cerberus_b200 import abi, synth, lib
-NW = int(sys.argv[1]) if len(sys.argv) > 1 else 148
+NW = int(sys.argv[1]) if len(sys.argv) > 1 else 132
 F = int(sys.argv[2]) if len(sys.argv) > 2 else 150
 REP = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 cfg = abi.default_config(); cfg.max_batch = NW; cfg.max_features = 160; cfg.max_obs = 160 * 11

@@ -1,5 +1,5 @@
-// tools/ubench.cu -- latency / throughput microbenchmarks of the fp64 building blocks of the solve kernel on sm_100a.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench tools/ubench.cu ; prints cycles per operation.
+// tools/ubench.cu -- latency / throughput microbenchmarks of the fp64 building blocks of the solve kernel on sm_90a.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench tools/ubench.cu ; prints cycles per operation.
 #include <cstdio>
 #include <cuda_runtime.h>
 #define DMMA(d0, d1, a, b, c0, c1) asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%4,%5};" : "=d"(d0), "=d"(d1) : "d"(a), "d"(b), "d"(c0), "d"(c1))

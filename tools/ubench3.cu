@@ -2,7 +2,7 @@
 // One CTA of 256 threads per SM (8 warps, two per scheduler, like vilo_solve_kernel).  Each warp runs either a DMMA stream (8 independent
 // accumulator chains) or an "evaluation-like" DFMA stream (4 independent chains of dependent FMAs + shared-memory loads); the time of each
 // role is reported for: all warps DFMA, all warps DMMA, one DMMA + one DFMA warp per scheduler, DMMA on schedulers 0-1 / DFMA on 2-3.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench3 tools/ubench3.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench3 tools/ubench3.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define DMMA(d0, d1, a, b, c0, c1) asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%4,%5};" : "=d"(d0), "=d"(d1) : "d"(a), "d"(b), "d"(c0), "d"(c1))
@@ -37,7 +37,7 @@ __global__ void k(double *out, long long *cyc, unsigned dmma_mask, int n_dmma, i
     out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
 }
 int main() {
-    double *out; long long *cyc; cudaMalloc(&out, 148 * 256 * 8); cudaMalloc(&cyc, 64);
+    double *out; long long *cyc; cudaMalloc(&out, 132 * 256 * 8); cudaMalloc(&cyc, 64);
     const int ND = 512, NF = 512;      // per warp: 4096 DMMA or 8192 DFMA (+ 1024 LDS.64)
     struct { const char *name; unsigned mask; } cases[] = {
         {"all 8 warps DFMA stream", 0x00}, {"all 8 warps DMMA stream", 0xff},
@@ -45,7 +45,7 @@ int main() {
         {"warp 0 DMMA only, 1-7 DFMA", 0x01}, {"warps 0-3 DMMA, 4-7 idle-ish (DFMA n=1)", 0x0f}};
     for (int c = 0; c < 6; c++) {
         long long h[8];
-        for (int rep = 0; rep < 2; rep++) { k<<<148, 256>>>(out, cyc, cases[c].mask, ND, c == 5 ? 1 : NF); cudaDeviceSynchronize(); }
+        for (int rep = 0; rep < 2; rep++) { k<<<132, 256>>>(out, cyc, cases[c].mask, ND, c == 5 ? 1 : NF); cudaDeviceSynchronize(); }
         cudaMemcpy(h, cyc, 64, cudaMemcpyDeviceToHost);
         printf("%-75s cycles per warp:", cases[c].name);
         for (int w = 0; w < 8; w++) printf(" %6lld%c", h[w], ((cases[c].mask >> w) & 1) ? 'T' : 'F');
