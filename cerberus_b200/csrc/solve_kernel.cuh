@@ -26,19 +26,25 @@ __device__ unsigned long long g_phase_cycles[48];
 #define PH_DECL() long long ph_t = clock64()
 #define PH_MARK_T(id, t) do { if ((threadIdx.x & 31) == 0) { const long long ph_n = clock64(); if (threadIdx.x == (t)) atomicAdd(&g_phase_cycles[id], (unsigned long long)(ph_n - ph_t)); ph_t = ph_n; } __syncwarp(); } while (0)
 #define PH_MARK(id) PH_MARK_T(id, 0)
+#define PH_ARG , long long &ph_t          // the phase functions of the solve kernel share the kernel's clock
+#define PH_FWD , ph_t
 #else
 #define PH_DECL()
 #define PH_MARK_T(id, t)
 #define PH_MARK(id)
+#define PH_ARG
+#define PH_FWD
 #endif
 
 enum { CERB_WINDOW = 10, NX = 79, NYB = 13, NFR = 11, NY = 143, NR = 222, NRP = 224, HXX_SZ = 79 * 79, HXY_SZ = 79 * 143, X_TD = 78, SOLVE_THREADS = 256, FT = 64, TILE_LD = 33, NOBS_PLANES = 9 };
+// block-tridiagonal Hyy: Ad = the NFR diagonal 13 x 13 blocks, Bo = the NFR - 1 blocks above the diagonal (row-major each)
+enum { HBLK = NYB * NYB, AD_SZ = NFR * HBLK, BO_SZ = (NFR - 1) * HBLK };
 #ifndef CERB_SOLVE_MIN_BLOCKS
 #define CERB_SOLVE_MIN_BLOCKS 1
 #endif
 // prior Hessian image in global memory: [Hxx (6241) | pad (1) | Hxy | Ad | Bo]: both parts start on 16-byte boundaries and have sizes that are
 // multiples of 16 bytes, so that each is ONE bulk copy (TMA 1-D, cp.async.bulk); shared memory has the same pad after Hxx (+ two mbarriers)
-enum { PIMG_HXY = HXX_SZ + 1, PIMG_REST = HXY_SZ + 1859 + 1690, PIMG_SZ = PIMG_HXY + PIMG_REST, SMEM_HXX_PAD = 3 };
+enum { PIMG_HXY = HXX_SZ + 1, PIMG_REST = HXY_SZ + AD_SZ + BO_SZ, PIMG_SZ = PIMG_HXY + PIMG_REST, SMEM_HXX_PAD = 3 };
 static_assert((PIMG_HXY * 8) % 16 == 0 && (PIMG_REST * 8) % 16 == 0 && ((HXX_SZ + SMEM_HXX_PAD) * 8) % 16 == 0, "bulk-copy alignment of the prior image");
 
 struct SolveParams {
@@ -63,12 +69,29 @@ struct SolveParams {
 };
 
 // per-CTA global workspace layout (doubles); F = maxF
-CERB_HD long ws_W(int) { return 0; }                                        // [NX][F]
 CERB_HD long ws_vecs(int F) { return (long)NX * F; }                        // 9 vectors of F: hh, gl, sl, Dl, ghl, gnl, stl, lamc, sinv (windows with > 1024 features)
 CERB_HD long ws_prior(int F) { return (long)NX * F + 9L * F; }              // image of the prior Hessian in the layout of Hxx | Hxy | Ad | Bo
 CERB_HD long ws_chunks(int F) { return ws_prior(F) + PIMG_SZ; }                          // feature chunk table (ints)
 CERB_HD long ws_imuplan(int F) { return (ws_chunks(F) + (F + 4) / 2 + 8 + 1) & ~1L; }                  // scatter plan of the IMU-leg Gram matrix (ints)
 CERB_HD long ws_size(int F) { return ws_imuplan(F) + 15 * 2 * 32 * 4 / 2 + 8; }                            // even: the plan is read as int4
+// this CTA's slice of the workspace
+struct CtaWs {
+    double *W, *hh, *gl, *sl, *Dl, *ghl, *gnl, *stl, *lamc, *sinv;     // sinv: 1 / sqrt(h + mu D^2) of windows with > 1024 features
+    int *chunks;                                                        // [0] n, [1..n] chunk starts, [n + 1] end of the last chunk
+    int *imu_plan;                                                      // scatter plan of the IMU-leg Gram matrix (build_imu_plan)
+    double *pimg;                                                       // prior Hessian image, built once per window
+    int F;                                                              // max_features: length of the vectors, leading dimension of W
+};
+CERB_D CtaWs ws_carve(const SolveParams &P) {
+    double *ws = P.ws + (size_t)blockIdx.x * P.ws_stride;
+    const int F = P.maxF;
+    CtaWs v;
+    v.W = ws;                                                           // [NX][F]
+    v.hh = ws + ws_vecs(F); v.gl = v.hh + F; v.sl = v.gl + F; v.Dl = v.sl + F; v.ghl = v.Dl + F; v.gnl = v.ghl + F; v.stl = v.gnl + F; v.lamc = v.stl + F; v.sinv = v.lamc + F;
+    v.chunks = reinterpret_cast<int *>(ws + ws_chunks(F)); v.imu_plan = reinterpret_cast<int *>(ws + ws_imuplan(F));
+    v.pimg = ws + ws_prior(F); v.F = F;
+    return v;
+}
 
 struct Smem {
     double *Hxx, *Hxy, *Ad, *Bo;            // 78x78, 78x143, 11x13x13, 10x13x13
@@ -80,24 +103,35 @@ struct Smem {
     double *pdx, *pr;                       // prior dx, residual (96 each)
     double *red;                            // 8 x 256 reduction scratch
     double *wj;                             // 128 x 8 per-thread exchange
-    double *sca;                            // 64 scalars
+    double *sca;                            // 32 scalars (S_*)
+    double *chain_col;                      // 2 x 16: double-buffered column line of the Hyy chain factorisation
     double *idg;                            // 143 (+pad): 1 / diag(L) of the block-bidiagonal factor of Hyy
     double *idx;                            // 79 (+pad): 1 / diag(L) of the dense factor of the reduced camera system
-    int *ti;                                // 128 ints: anchor per tile factor ; + misc ints
+    int *ti;                                // TI_INTS ints (TI_*)
     unsigned long long *mbar;               // two mbarriers (bulk copies of the prior image: [0] Hxx part, [1] Hxy | Ad | Bo part)
     double *tile;                           // alias of Hxy (+ Ad, Bo): 256 x TILE_LD tile + 8 x 640 partial Gram tiles
 };
-enum { SMEM_DOUBLES = HXX_SZ + SMEM_HXX_PAD + HXY_SZ + 1859 + 1690 + 7 * NRP + 2 * ST_STRIDE + 99 + 18 + 3 + 31 * 39 + 960 + 192 + 8 * 256 + 128 * 8 + 64 + 66 + 144 + 80 };
+// scalar slots of s.sca
+enum { S_RADIUS = 0, S_MU, S_REUSE, S_XCOST, S_CCOST, S_ALPHA, S_GNORM2, S_GNNORM2, S_GDOTGN, S_MODEL, S_STEPNORM, S_XNORM, S_DLNORM,
+       S_OK, S_DONE, S_TERM, S_ITER, S_NSUCC, S_INVALID, S_GMAX, S_INIT_COST, S_P, S_Q, S_VHV, S_LCOST, S_LNORM, S_LGMAX, S_COUNT };
+static_assert(S_COUNT <= 32, "scalar slots overlap the chain's column line");
+// int slots of s.ti: the prior's column -> destination map from 0 (build_prior_image), the feature chunk count, the first
+// TI_CACHED_CHUNKS chunks as (start, count << 8 | anchor) pairs (build_chunks), the number of Hyy blocks the chain factorisation has
+// published, the IMU-leg factor mask (0: all factors, 1: only factor 0, 2: none)
+enum { TI_PRIOR_MAP = 0, TI_NCHUNKS = 96, TI_CHUNK_CACHE = 97, TI_CACHED_CHUNKS = 15, TI_CHAIN_DONE = 130, TI_IMU_MASK = 131, TI_INTS = 132 };
+static_assert(TI_PRIOR_MAP + CERB_MAX_PRIOR_DIM <= TI_NCHUNKS && TI_CHUNK_CACHE + 2 * TI_CACHED_CHUNKS <= TI_CHAIN_DONE && TI_IMU_MASK < TI_INTS && TI_INTS % 2 == 0,
+              "s.ti slots overlap");
+enum { SMEM_DOUBLES = HXX_SZ + SMEM_HXX_PAD + HXY_SZ + AD_SZ + BO_SZ + 7 * NRP + 2 * ST_STRIDE + 99 + 18 + 3 + 31 * 39 + 960 + 192 + 8 * 256 + 128 * 8 + 32 + 32 + TI_INTS / 2 + 144 + 80 };
 
 CERB_D void smem_carve(double *base, Smem &s) {
     double *p = base;
-    s.Hxx = p; p += HXX_SZ; s.mbar = reinterpret_cast<unsigned long long *>(p + 1); p += SMEM_HXX_PAD; s.Hxy = p; p += HXY_SZ; s.Ad = p; p += 1859; s.Bo = p; p += 1690;
+    s.Hxx = p; p += HXX_SZ; s.mbar = reinterpret_cast<unsigned long long *>(p + 1); p += SMEM_HXX_PAD; s.Hxy = p; p += HXY_SZ; s.Ad = p; p += AD_SZ; s.Bo = p; p += BO_SZ;
     s.g = p; p += NRP; s.sc = p; p += NRP; s.D = p; p += NRP; s.gh = p; p += NRP; s.gn = p; p += NRP; s.stp = p; p += NRP; s.yv = p; p += NRP;
     s.xs = p; p += ST_STRIDE; s.xc = p; p += ST_STRIDE;
     s.Rw = p; p += 99; s.Rex = p; p += 18; p += 3;
     s.Ju = p; p += 31 * 39; s.red = p; p += 8 * 256; s.wj = p; p += 128 * 8;      // contiguous scratch (4281 doubles): IMU_SCRATCH, Schur tile
-    s.lin = p; p += 960; s.pdx = p; p += 96; s.pr = p; p += 96; s.sca = p; p += 64;
-    s.ti = reinterpret_cast<int *>(p); p += 66;       // 132 ints
+    s.lin = p; p += 960; s.pdx = p; p += 96; s.pr = p; p += 96; s.sca = p; p += 32; s.chain_col = p; p += 32;
+    s.ti = reinterpret_cast<int *>(p); p += TI_INTS / 2;
     s.idg = p; p += 144;
     s.idx = p; p += 80;
     s.tile = s.Hxy;
@@ -264,10 +298,10 @@ CERB_NOINLINE double vision_linearize(const SolveParams &P, int w, const double 
     for (int g = 0; g < 4; g++) { const int pc = g == 0 ? c8 : 8 + 6 * (g - 1) + c8; tv[g] = (g == 0) || c8 < 6; tq[g] = T + (tv[g] ? pc : 0) * VT_LD + (lane & 3); }
     int jbase, jca, jcj;                                                // scatter plan of this thread's entry of the frame-dependent blocks
     vis_jplan(s, smem_base, tid, &jbase, &jca, &jcj);
-    const int nchunks = s.ti[96];
+    const int nchunks = s.ti[TI_NCHUNKS];
     for (int ch = 0; ch < nchunks; ch++) {
         int c0, nc, a;                                                  // chunk table: shared-memory cache (no dependent L2 round trips), else global
-        if (ch < 15) { c0 = s.ti[97 + 2 * ch]; nc = s.ti[98 + 2 * ch] >> 8; a = s.ti[98 + 2 * ch] & 255; }
+        if (ch < TI_CACHED_CHUNKS) { const int *cc = s.ti + TI_CHUNK_CACHE + 2 * ch; c0 = cc[0]; nc = cc[1] >> 8; a = cc[1] & 255; }
         else { c0 = chunks[1 + ch]; nc = chunks[2 + ch] - c0; a = P.feat_start[(size_t)w * F + c0]; }
         const int f = c0 + fl;
         const bool ev = fl < nc;
@@ -586,9 +620,9 @@ CERB_D void scatter_addr(const Smem &s, int da, int db, double **a0, double **a1
     if (db >= 0) { *a0 = s.Hxy + db * NY + (-da - 1); return; }
     const int ya = -da - 1, yb = -db - 1;
     const int fa = ya / NYB, fb = yb / NYB, ka = ya % NYB, kb = yb % NYB;
-    if (fa == fb) { *a0 = s.Ad + fa * 169 + ka * NYB + kb; if (ka != kb) *a1 = s.Ad + fa * 169 + kb * NYB + ka; }
-    else if (fb == fa + 1) *a0 = s.Bo + fa * 169 + ka * NYB + kb;
-    else *a0 = s.Bo + fb * 169 + kb * NYB + ka;
+    if (fa == fb) { *a0 = s.Ad + fa * HBLK + ka * NYB + kb; if (ka != kb) *a1 = s.Ad + fa * HBLK + kb * NYB + ka; }
+    else if (fb == fa + 1) *a0 = s.Bo + fa * HBLK + ka * NYB + kb;
+    else *a0 = s.Bo + fb * HBLK + kb * NYB + ka;
 }
 CERB_D void scatter_H(Smem &s, int da, int db, double v) {
     if (da >= 0 && db >= 0) { if (da <= db) s.Hxx[da * NX + db] += v; else s.Hxx[db * NX + da] += v; return; }
@@ -596,9 +630,9 @@ CERB_D void scatter_H(Smem &s, int da, int db, double v) {
     if (db >= 0) { s.Hxy[db * NY + (-da - 1)] += v; return; }
     const int ya = -da - 1, yb = -db - 1;
     const int fa = ya / NYB, fb = yb / NYB, ka = ya % NYB, kb = yb % NYB;
-    if (fa == fb) { s.Ad[fa * 169 + ka * NYB + kb] += v; if (ka != kb) s.Ad[fa * 169 + kb * NYB + ka] += v; }
-    else if (fb == fa + 1) s.Bo[fa * 169 + ka * NYB + kb] += v;
-    else s.Bo[fb * 169 + kb * NYB + ka] += v;
+    if (fa == fb) { s.Ad[fa * HBLK + ka * NYB + kb] += v; if (ka != kb) s.Ad[fa * HBLK + kb * NYB + ka] += v; }
+    else if (fb == fa + 1) s.Bo[fa * HBLK + ka * NYB + kb] += v;
+    else s.Bo[fb * HBLK + kb * NYB + ka] += v;
 }
 
 // Inertial linearisation.  Warps 0..2 each run whole IMU-leg factors on their own (warp-synchronous, no block barriers):
@@ -630,7 +664,7 @@ CERB_NOINLINE double inertial_linearize(const SolveParams &P, int w, const doubl
         // scatter plan of this lane (built once per launch), kept in registers: x = offset(i = 0), y = stride | (mirror delta + 256) << 12
         int plx[30], ply[30];
         {
-            const int *plan = reinterpret_cast<const int *>(P.ws + (size_t)blockIdx.x * P.ws_stride + ws_imuplan(P.maxF));
+            const int *plan = ws_carve(P).imu_plan;
             _Pragma("unroll")
             for (int q = 0; q < 30; q++) { plx[q] = __ldg(plan + (2 * q) * 32 + lane); ply[q] = __ldg(plan + (2 * q + 1) * 32 + lane); }
             // entries without a destination share a dummy slot per lane in the plan: give every IMU warp its own (no write-write hazard between warps)
@@ -651,7 +685,7 @@ CERB_NOINLINE double inertial_linearize(const SolveParams &P, int w, const doubl
                 }
         };
         load_S(wid * 4);
-        const int imu_mask = s.ti[131];                                   // 0: all factors (solve); marginalization: 1 only factor 0, 2 none
+        const int imu_mask = s.ti[TI_IMU_MASK];                           // 0: all factors (solve); marginalization: 1 only factor 0, 2 none
         double sdt[4];                                                    // sum_dt of this warp's factors, fetched up front
         _Pragma("unroll")
         for (int rnd = 0; rnd < 4; rnd++) { const int i = rnd + 4 * wid; sdt[rnd] = (i < CERB_WINDOW) ? P.pre[((size_t)w * CERB_WINDOW + i) * PRE_STRIDE + PRE_SUM_DT] : 1e30; }
@@ -757,8 +791,8 @@ CERB_NOINLINE double inertial_linearize(const SolveParams &P, int w, const doubl
                 double t = 0.0;
                 for (int k = lane; k < n; k += 32) t += J[(size_t)c * n + k] * s.pr[k];
                 for (int o = 16; o > 0; o >>= 1) t += __shfl_sync(0xffffffffu, t, (lane + o) & 31);
-                const int d = s.ti[c];
-                if (lane == 0 && d != (1 << 20)) gp[d >= 0 ? d : NX + (-d - 1)] += t;
+                const int d = s.ti[TI_PRIOR_MAP + c];                  // the kept blocks tile all n columns (validate_prior)
+                if (lane == 0) gp[d >= 0 ? d : NX + (-d - 1)] += t;
             }
         }
         PH_MARK_T(31, 96);
@@ -904,8 +938,8 @@ template <int W> CERB_D void schur_scatter(Smem &s, const double (&acc)[8][2], i
     }
 }
 
-// prior Hessian image (J0^T J0 scattered into the layout of Hxx | Hxy | Ad | Bo) in global memory + the column -> destination map of
-// the prior in s.ti[0..n); returns whether the window has a prior
+// prior Hessian image (J0^T J0 scattered into the layout of Hxx | Hxy | Ad | Bo) in global memory: constant during the solve, every linearisation
+// starts from it instead of from zero; + the column -> destination map of the prior in s.ti[TI_PRIOR_MAP + 0..n); returns whether the window has a prior
 CERB_D bool build_prior_image(const SolveParams &P, Smem &s, int w, double *pimg, int tid) {
     const int *pmeta = P.prior_meta + (size_t)w * PRIOR_META_STRIDE;
     const bool has_prior = pmeta[0] != 0;
@@ -922,19 +956,652 @@ CERB_D bool build_prior_image(const SolveParams &P, Smem &s, int w, double *pimg
                 else if (kind == 1) d = -(1 + NYB * index + k);
                 else if (kind == 2) d = -(1 + NYB * index + 9 + k);
                 else d = X_TD;
-                s.ti[col + k] = d;
+                s.ti[TI_PRIOR_MAP + col + k] = d;
             }
         }
         __syncthreads();
-        Smem si = s; si.Hxx = pimg; si.Hxy = pimg + PIMG_HXY; si.Ad = pimg + PIMG_HXY + HXY_SZ; si.Bo = pimg + PIMG_HXY + HXY_SZ + 1859;
+        Smem si = s; si.Hxx = pimg; si.Hxy = pimg + PIMG_HXY; si.Ad = pimg + PIMG_HXY + HXY_SZ; si.Bo = pimg + PIMG_HXY + HXY_SZ + AD_SZ;
         const double *Hp = P.prior_Hp + (size_t)w * PRIOR_LD * PRIOR_LD;
         for (int idx = tid; idx < n * n; idx += SOLVE_THREADS) {
             const int a = idx / n, b = idx % n;
             if (b < a) continue;
-            scatter_H(si, s.ti[a], s.ti[b], Hp[a * PRIOR_LD + b]);
+            scatter_H(si, s.ti[TI_PRIOR_MAP + a], s.ti[TI_PRIOR_MAP + b], Hp[a * PRIOR_LD + b]);
         }
     }
     return has_prior;
+}
+
+// ---- the prologue both kernels share ----------------------------------------------------------------------------
+// Scatter plan of the 40 x 40 IMU-leg Gram matrix (inertial_linearize), built by warp 0 once per launch: lane `tid` holds, for block
+// q = (mi, ni) and e = 0, 1, the entry (la, lb) = (8 mi + lane / 4, 8 ni + 2 (lane % 4) + e).  Its destination in Hxx / Hxy / Hyy / g is
+// affine in the factor index i, so the plan stores two ints: offset(i = 0) and stride | (mirror delta + 256) << 12 (in doubles
+// from the start of shared memory; the mirror is the transposed entry of a diagonal Hyy block).  Entries without a destination
+// point at a per-lane dummy slot (idg[32 warp + lane], never read) with stride 0.
+CERB_D void build_imu_plan(const Smem &s, const double *smem_base, int *plan, int tid) {
+    if (tid >= 32) return;
+    int q = 0;
+    for (int mi = 0; mi < 5; mi++)
+        for (int ni = mi; ni < 5; ni++, q++)
+            for (int e = 0; e < 2; e++) {
+                const int la = 8 * mi + (tid >> 2), lb = 8 * ni + 2 * (tid & 3) + e;
+                int px = (int)(s.idg - smem_base) + tid, py = 256 << 12;         // default: dummy slot of this lane (idg is idle during a linearisation; each IMU warp adds 32 x its index), stride 0, delta 0
+                if (la <= lb && lb <= 38 && la != 38) {
+                    double *p0[2], *p1[2];
+                    for (int i = 0; i < 2; i++) {
+                        const int da = imu_col_dest(i, la);
+                        if (lb == 38) { p0[i] = da >= 0 ? s.g + da : s.g + NX + (-da - 1); p1[i] = nullptr; }
+                        else scatter_addr(s, da, imu_col_dest(i, lb), &p0[i], &p1[i]);
+                    }
+                    px = (int)(p0[0] - smem_base);
+                    py = (int)(p0[1] - p0[0]) | (((p1[0] ? (int)(p1[0] - p0[0]) : 0) + 256) << 12);
+                }
+                plan[(2 * (q * 2 + e)) * 32 + tid] = px; plan[(2 * (q * 2 + e) + 1) * 32 + tid] = py;
+            }
+}
+// feature chunks of the tracks [0, n_end) (anchor frames fstart) for vision_linearize (one thread): <= 64 consecutive tracks with the same anchor frame
+CERB_D void build_chunks(const int *fstart, Smem &s, int *chunks, int n_end) {
+    int n = 0, c0 = 0;
+    while (c0 < n_end) {
+        chunks[1 + n] = c0;
+        const int a = fstart[c0];
+        int e = c0 + 1;
+        while (e < n_end && e < c0 + 64 && fstart[e] == a) e++;
+        if (n < TI_CACHED_CHUNKS) { s.ti[TI_CHUNK_CACHE + 2 * n] = c0; s.ti[TI_CHUNK_CACHE + 2 * n + 1] = ((e - c0) << 8) | a; }   // also cached in shared memory
+        n++; c0 = e;
+    }
+    chunks[1 + n] = n_end; chunks[0] = n; s.ti[TI_NCHUNKS] = n;
+}
+// ---- the solve kernel: the window of a CTA and the phases of one trust-region iteration ---------------------------
+struct Win { int w, nF; bool ex_open, lb_open, td_open, has_prior, bulk_ok; double *lam; CtaWs ws; };     // lam: inverse depths of the current point
+struct PriorCopy { unsigned par0, par1; bool hxx_prefetched; };    // prior-image copies: parities of the two bulk-copy mbarriers, Hxx part in flight
+// linearisation at (xl, laml): H, g (Jacobi scaled), W, hh, gl; results S_LCOST (cost), S_LNORM (||x||), S_LGMAX (max |g|)
+CERB_D void linearize(const SolveParams &P, Smem &s, const Win &c, PriorCopy &pc, const double *xl, const double *laml, bool first, int tid PH_ARG) {
+    const int F = c.ws.F, nF = c.nF;
+    double *sca = s.sca, *W = c.ws.W, *hh = c.ws.hh, *gl = c.ws.gl, *sl = c.ws.sl, *pimg = c.ws.pimg;
+    // start from the prior Hessian image; its Hxx part was prefetched asynchronously when the previous factorisation of
+    // Hxx had been consumed (the copy overlapped with the rest of that iteration), except for the first linearisation
+    if (!c.has_prior) { for (int k = tid; k < HXX_SZ; k += SOLVE_THREADS) s.Hxx[k] = 0.0; }
+    else if (c.bulk_ok) {
+        if (!pc.hxx_prefetched) { __syncthreads(); if (tid == 0) CERB_BULK_G2S(s.Hxx, pimg, PIMG_HXY * 8, &s.mbar[0]); }
+        CERB_MBAR_WAIT(&s.mbar[0], pc.par0); pc.par0 ^= 1;
+    } else { if (!pc.hxx_prefetched) copy_g2s_async(s.Hxx, pimg, HXX_SZ, tid); CERB_CP_ASYNC_WAIT(); }
+    pc.hxx_prefetched = false;
+    for (int k = tid; k < NRP; k += SOLVE_THREADS) s.g[k] = 0.0;
+    load_geometry(xl, s, tid);
+    double part[2];
+    PH_MARK(0);
+    part[0] = vision_linearize(P, c.w, xl, laml, W, hh, gl, sl, !first, c.ws.chunks, tid);
+    if (c.has_prior && c.bulk_ok) {                                                              // Hxy | Ad | Bo (contiguous; the tile aliased them):
+        if (tid == 0) CERB_BULK_G2S(s.Hxy, pimg + PIMG_HXY, PIMG_REST * 8, &s.mbar[1]);            // one bulk copy (vision_linearize ended with a barrier)
+        CERB_MBAR_WAIT(&s.mbar[1], pc.par1); pc.par1 ^= 1;
+    } else if (c.has_prior) copy_g2s_async(s.Hxy, pimg + PIMG_HXY, PIMG_REST, tid);               // completed inside inertial_linearize
+    else for (int k = tid; k < PIMG_REST; k += SOLVE_THREADS) s.Hxy[k] = 0.0;
+    __syncthreads();
+    PH_MARK(1);
+    part[0] += inertial_linearize(P, c.w, xl, tid);
+    PH_MARK(2);
+    part[1] = ambient_sq(xl, nullptr, laml, nullptr, nF, c.ex_open, c.lb_open, c.td_open, tid);
+    double tot[2];
+    block_sum<2>(part, s.red, tot, tid);
+    if (tid == 0) { sca[S_LCOST] = tot[0]; sca[S_LNORM] = sqrt(tot[1]); }
+    // (Hxx holds its upper triangle; it is mirrored and scaled in one row-wise pass below)
+    // gradient max norm over active dims (unscaled), Jacobi scale at the first linearisation
+    if (first) {
+        for (int k = tid; k < NR; k += SOLVE_THREADS) {
+            double d;
+            bool active = true;
+            if (k < NX) { d = s.Hxx[k * NX + k]; if (k >= 66 && k < X_TD && !c.ex_open) active = false; if (k == X_TD && !c.td_open) active = false; }
+            else { const int yk = k - NX, f = yk / NYB, q = yk % NYB; d = s.Ad[f * HBLK + q * NYB + q]; if (q >= 9 && !c.lb_open) active = false; }
+            s.sc[k] = active ? 1.0 / (1.0 + sqrt(d)) : 0.0;
+        }
+        for (int f = tid; f < nF; f += SOLVE_THREADS) sl[f] = 1.0 / (1.0 + sqrt(hh[f]));
+    }
+    __syncthreads();
+    if (P.dbg && c.w == P.dbg_window && first) {      // parity probe, ABI order
+        for (int k = tid; k < NR; k += SOLVE_THREADS) {
+            int dst; double d;
+            if (k < NX) { dst = k < X_TD ? k : 221; d = s.Hxx[k * NX + k]; }      // ABI order: td after the leg biases
+            else { const int yk = k - NX, f = yk / NYB, q = yk % NYB; dst = q < 9 ? 78 + 9 * f + q : 177 + 4 * f + (q - 9); d = s.Ad[f * HBLK + q * NYB + q]; }
+            const bool act = s.sc[k] != 0.0;
+            P.dbg[1 + dst] = act ? s.g[k] : 0.0; P.dbg[1 + NR + F + dst] = act ? d : 0.0;
+        }
+        for (int f = tid; f < nF; f += SOLVE_THREADS) { P.dbg[1 + NR + f] = gl[f]; P.dbg[1 + NR + F + NR + f] = hh[f]; }
+        if (tid == 0) P.dbg[0] = sca[S_LCOST];
+    }
+    double gm = 0.0;
+    for (int k = tid; k < NR; k += SOLVE_THREADS) if (s.sc[k] != 0.0) gm = fmax(gm, fabs(s.g[k]));
+    for (int f = tid; f < nF; f += SOLVE_THREADS) gm = fmax(gm, fabs(!first ? gl[f] / sl[f] : gl[f]));   // unscaled gradient
+    for (int o = 16; o > 0; o >>= 1) gm = fmax(gm, __shfl_sync(0xffffffffu, gm, (tid + o) & 31));
+    if ((tid & 31) == 0) s.red[tid >> 5] = gm;
+    __syncthreads();
+    if (tid == 0) { double m8 = s.red[0]; for (int k = 1; k < SOLVE_THREADS / 32; k++) m8 = fmax(m8, s.red[k]); sca[S_LGMAX] = m8; }
+    // apply the Jacobi scaling: H~ = S H S, g~ = S g, w~_f = s_f S_x w_f, h~ = s_f^2 h, gl~ = s_f gl.  Row-wise (a warp per
+    // row: no index divisions); the Hxx pass also mirrors the upper triangle into the lower one.
+    for (int a = tid >> 5; a < NX; a += SOLVE_THREADS / 32) {
+        const double sa = s.sc[a];
+        for (int b = a + (tid & 31); b < NX; b += 32) { const double v = s.Hxx[a * NX + b] * (sa * s.sc[b]); s.Hxx[a * NX + b] = v; s.Hxx[b * NX + a] = v; }
+        for (int q = tid & 31; q < NY; q += 32) s.Hxy[a * NY + q] *= sa * s.sc[NX + q];
+    }
+    for (int k = tid; k < AD_SZ; k += SOLVE_THREADS) { const int f = k / HBLK, a = (k % HBLK) / NYB, b = k % NYB; s.Ad[k] *= s.sc[NX + NYB * f + a] * s.sc[NX + NYB * f + b]; }
+    for (int k = tid; k < BO_SZ; k += SOLVE_THREADS) { const int f = k / HBLK, a = (k % HBLK) / NYB, b = k % NYB; s.Bo[k] *= s.sc[NX + NYB * f + a] * s.sc[NX + NYB * (f + 1) + b]; }
+    for (int k = tid; k < NR; k += SOLVE_THREADS) s.g[k] *= s.sc[k];
+    if (first) {      // later linearisations write W, hh, gl pre-scaled
+        for (int k = tid; k < NX * nF; k += SOLVE_THREADS) { const int a = k / nF, f = k % nF; W[(size_t)a * F + f] *= s.sc[a] * sl[f]; }
+        for (int f = tid; f < nF; f += SOLVE_THREADS) { hh[f] *= sl[f] * sl[f]; gl[f] *= sl[f]; }
+    }
+    __syncthreads();
+}
+// FinalizeIterationAndCheckIfMinimizerCanContinue; true: the minimizer stops
+CERB_D bool finalize_iteration(const SolveParams &P, double *sca, int iteration, int tid) {
+    if (tid == 0) {
+        if (iteration >= P.max_iters) { sca[S_DONE] = 1; sca[S_TERM] = 1; }
+        else if (sca[S_GMAX] <= P.gtol) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
+        else if (sca[S_RADIUS] <= P.min_radius) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
+        else if (!(sca[S_XCOST] == sca[S_XCOST]) || fabs(sca[S_XCOST]) > 1e300) { sca[S_DONE] = 1; sca[S_TERM] = 2; }
+    }
+    __syncthreads();
+    return sca[S_DONE] != 0.0;
+}
+// dogleg diagonal D, gradient / D, scaled gradient v (kept in s.stp: the Cauchy point's v^T H v is finished in lambda_schur);
+// ||gh||^2 and the Hyy part of v^T H v (Hyy is about to be factored in place)
+CERB_D void dogleg_diagonal(Smem &s, const Win &c, int tid PH_ARG) {
+    const int nF = c.nF;
+    double *sca = s.sca, *Dl = c.ws.Dl, *ghl = c.ws.ghl, *stl = c.ws.stl;
+    for (int k = tid; k < NR; k += SOLVE_THREADS) {
+        const double d = (k < NX) ? s.Hxx[k * NX + k] : s.Ad[((k - NX) / NYB) * HBLK + ((k - NX) % NYB) * (NYB + 1)];
+        const double D = sqrt(fmin(fmax(d, 1e-6), 1e32));
+        s.D[k] = D; s.gh[k] = s.g[k] / D; s.stp[k] = s.gh[k] / D;
+    }
+    for (int f = tid; f < nF; f += SOLVE_THREADS) { const double D = sqrt(fmin(fmax(c.ws.hh[f], 1e-6), 1e32)); Dl[f] = D; ghl[f] = c.ws.gl[f] / D; stl[f] = ghl[f] / D; }
+    __syncthreads();
+    double part[2] = {0.0, 0.0};     // [0] v_y^T Hyy v_y  [1] ||gh||^2
+    for (int k = tid; k < AD_SZ; k += SOLVE_THREADS) { const int f = k / HBLK, a = (k % HBLK) / NYB, b = k % NYB; part[0] += s.stp[NX + NYB * f + a] * s.Ad[k] * s.stp[NX + NYB * f + b]; }
+    for (int k = tid; k < BO_SZ; k += SOLVE_THREADS) { const int f = k / HBLK, a = (k % HBLK) / NYB, b = k % NYB; part[0] += 2.0 * s.stp[NX + NYB * f + a] * s.Bo[k] * s.stp[NX + NYB * (f + 1) + b]; }
+    for (int f = tid; f < nF; f += SOLVE_THREADS) part[1] += ghl[f] * ghl[f];
+    for (int k = tid; k < NR; k += SOLVE_THREADS) part[1] += s.gh[k] * s.gh[k];
+    double tot[2];
+    block_sum<2>(part, s.red, tot, tid);
+    if (tid == 0) { sca[S_GNORM2] = tot[1]; sca[S_VHV] = tot[0]; sca[S_OK] = 1; }      // S_OK: a failure below is an invalid step: mu *= 10, re-linearise
+    PH_MARK(4);
+}
+// warp 0: block-bidiagonal Cholesky of Hyy: Ad[f] <- L_f (lower), Bo[f] <- M_f = B_f^T L_f^-T.  Lane r owns row r of the 13 x 13 block in
+// registers; the column sweep exchanges pivots and column entries with shuffles (no shared-memory round trips on the dependency chain).
+// Every finished block f is published through chain_done = f + 1.
+CERB_D void chain_cholesky(Smem &s, int *chain_done, int lane PH_ARG) {
+    const bool act = lane < NYB;
+    const int r = act ? lane : 0;              // idle lanes shadow row 0 and never store
+    double m[NYB];                             // row r of M_{f-1}
+    _Pragma("unroll")
+    for (int c = 0; c < NYB; c++) m[c] = 0.0;
+    _Pragma("unroll 1")                        // keep the block body compact: it is re-used 11 times from the instruction cache
+    for (int f = 0; f < NFR; f++) {
+        double *A = s.Ad + f * HBLK;
+        double a[NYB], invd[NYB], myinv = 1.0;
+        _Pragma("unroll")
+        for (int c = 0; c < NYB; c++) a[c] = A[r * NYB + c];
+        if (f > 0) {
+            const double *Mp = s.Bo + (f - 1) * HBLK;        // M[r][c], r: y_f index, c: y_{f-1} index
+            _Pragma("unroll")
+            for (int c = 0; c < NYB; c++) { double t = 0.0; _Pragma("unroll") for (int q = 0; q < NYB; q++) t += m[q] * Mp[c * NYB + q]; a[c] -= t; }
+        }
+        _Pragma("unroll")
+        for (int j = 0; j < NYB; j++) {                     // right-looking column sweep
+            double d = __shfl_sync(0xffffffffu, a[j], j);
+            if (!(d > 0.0)) { if (lane == 0) s.sca[S_OK] = 0; d = 1.0; }
+            const double inv = rsqrt(d);
+            invd[j] = inv;
+            if (lane == j) myinv = inv;
+            const double l = (lane == j) ? d * inv : a[j] * inv;
+            a[j] = l;
+            // column j of L to all lanes through a double-buffered shared-memory line (1 store + 12 broadcast loads
+            // instead of 12 two-instruction shuffles: the sweep is bound by the instruction issue of this one warp)
+            double *colb = s.chain_col + 16 * (j & 1);
+            if (act) colb[lane] = l;
+            __syncwarp();
+            _Pragma("unroll")
+            for (int k = j + 1; k < NYB; k++) a[k] -= l * colb[k];
+        }
+        if (act) { _Pragma("unroll") for (int c = 0; c < NYB; c++) if (c <= r) A[r * NYB + c] = a[c]; s.idg[NYB * f + r] = myinv; }
+        __syncwarp();
+        if (f < NFR - 1) {
+            double *B = s.Bo + f * HBLK;                     // in: B[k1][k2] = H(y_f[k1], y_{f+1}[k2]); out: M[r][c]
+            double t[NYB];
+            _Pragma("unroll")
+            for (int c = 0; c < NYB; c++) t[c] = B[c * NYB + r];
+            _Pragma("unroll")
+            for (int c = 0; c < NYB; c++) {
+                m[c] = t[c] * invd[c];
+                _Pragma("unroll")
+                for (int c2 = c + 1; c2 < NYB; c2++) t[c2] -= m[c] * A[c2 * NYB + c];
+            }
+            __syncwarp();
+            if (act) { _Pragma("unroll") for (int c = 0; c < NYB; c++) B[r * NYB + c] = m[c]; }
+            __syncwarp();
+        }
+        __threadfence_block(); __syncwarp();
+        if (lane == 0) CERB_ST_RELEASE_S32(chain_done, f + 1);   // L_f, M_f and the inverse pivots of block f are in shared memory
+    }
+    PH_MARK(6);
+}
+// warp-uniform dispatch to the compile-time block plans (SCPlan, TTPlan)
+CERB_D void schur_tile_w(int wq, const double *tw, double (&acc)[8][2], int lane) {
+    switch (wq) { case 0: schur_tile<0>(tw, acc, lane); break; case 1: schur_tile<1>(tw, acc, lane); break; case 2: schur_tile<2>(tw, acc, lane); break;
+                  case 3: schur_tile<3>(tw, acc, lane); break; case 4: schur_tile<4>(tw, acc, lane); break; case 5: schur_tile<5>(tw, acc, lane); break;
+                  default: schur_tile<6>(tw, acc, lane); break; }
+}
+CERB_D void schur_scatter_w(int wq, Smem &s, const double (&acc)[8][2], int lane) {
+    switch (wq) { case 0: schur_scatter<0>(s, acc, lane); break; case 1: schur_scatter<1>(s, acc, lane); break; case 2: schur_scatter<2>(s, acc, lane); break;
+                  case 3: schur_scatter<3>(s, acc, lane); break; case 4: schur_scatter<4>(s, acc, lane); break; case 5: schur_scatter<5>(s, acc, lane); break;
+                  default: schur_scatter<6>(s, acc, lane); break; }
+}
+CERB_D void ttt_warp_w(int wq, Smem &s, int lane) {
+    switch (wq) { case 0: ttt_warp<0>(s, lane); break; case 1: ttt_warp<1>(s, lane); break; case 2: ttt_warp<2>(s, lane); break; case 3: ttt_warp<3>(s, lane); break;
+                  case 4: ttt_warp<4>(s, lane); break; case 5: ttt_warp<5>(s, lane); break; case 6: ttt_warp<6>(s, lane); break; default: ttt_warp<7>(s, lane); break; }
+}
+// warps 1..7: the Cauchy point's v_x^T Hxx v_x + 2 v_x^T Hxy v_y + lambda terms (into s.lin[0..7)), the mu-regularised diagonal of Hxx,
+// then the inverse depths are eliminated on the fp64 tensor cores:
+//   S = Hxx - W' W'^T,  rhs_x -= W' (w g_l),  W'[a][f] = W[a][f] / sqrt(h_f + mu D_f^2)
+// W' is staged through shared memory 32 features at a time as an 80-row tile whose row 78 carries
+// g_l / sqrt(h + mu D^2) (so that column 78 of the Gram matrix is the rhs update) and row 79 is zero.
+// The 55 upper 8x8 blocks of the 80x80 Gram matrix go to the 7 warps as row strips (SCPlan, compile-time).
+CERB_D void lambda_schur(Smem &s, const Win &c, double mu, int tid PH_ARG) {
+    const int F = c.ws.F, nF = c.nF;
+    const double *W = c.ws.W, *hh = c.ws.hh, *gl = c.ws.gl, *Dl = c.ws.Dl, *stl = c.ws.stl;
+    const int t2 = tid - 32, n2 = SOLVE_THREADS - 32;
+    const int wq = (tid >> 5) - 1, lane = tid & 31;
+    const int LDW = SC_LDW;
+    double *tw = s.Ju;                         // 80 x 36 tile (aliases Ju .. red, unused during the solve)
+    double *sinv = nF <= 1024 ? s.wj : c.ws.sinv;  // 1 / sqrt(h + mu D^2): shared memory (wj: 1024 doubles) up to the reference's NUM_OF_F,
+                                                   // the ninth workspace vector for the larger synthetic stress windows
+    {   // Cauchy point (H still unregularised / unfactored here)
+        const double *v = s.stp;
+        double pv = 0.0;
+        for (int k = t2; k < NX * NX; k += n2) pv += v[k / NX] * s.Hxx[k] * v[k % NX];
+        for (int k = t2; k < NX * NY; k += n2) pv += 2.0 * v[k / NY] * s.Hxy[k] * v[NX + k % NY];
+        for (int f = t2; f < nF; f += n2) {
+            double wv = 0.0;
+            for (int a = 0; a < NX; a++) wv += W[(size_t)a * F + f] * v[a];
+            pv += 2.0 * stl[f] * wv + hh[f] * stl[f] * stl[f];
+        }
+        for (int o = 16; o > 0; o >>= 1) pv += __shfl_sync(0xffffffffu, pv, (lane + o) & 31);
+        if (lane == 0) s.lin[wq] = pv;
+        CERB_BAR_SYNC(1, n2);
+        for (int k = t2; k < NX; k += n2) s.Hxx[k * NX + k] += mu * s.D[k] * s.D[k];
+    }
+    PH_MARK_T(19, 32);
+    for (int f = t2; f < nF; f += n2) sinv[f] = rsqrt(hh[f] + mu * Dl[f] * Dl[f]);
+    double acc[8][2];
+    _Pragma("unroll")
+    for (int k = 0; k < 8; k++) { acc[k][0] = 0.0; acc[k][1] = 0.0; }
+    CERB_BAR_SYNC(1, n2);
+    // raw W / g_l values of a tile are fetched into registers one tile ahead (12 per thread: the loads are issued
+    // together and stay in flight during the tensor-core loop), scaled and stored when the tile buffer is free
+    double buf[12];
+    auto fetch = [&](int f0) {
+        const int nf = (nF - f0) < 32 ? (nF - f0) : 32;
+        _Pragma("unroll")
+        for (int u = 0; u < 12; u++) {
+            const int e = t2 + u * n2, a = e >> 5, f = e & 31;
+            buf[u] = (e < 80 * 32 && f < nf) ? (a < NX ? W[(size_t)a * F + f0 + f] : (a == NX ? gl[f0 + f] : 0.0)) : 0.0;
+        }
+    };
+    fetch(0);
+    PH_MARK_T(37, 32);
+    for (int f0 = 0; f0 < nF; f0 += 32) {
+        const int nf = (nF - f0) < 32 ? (nF - f0) : 32;
+        _Pragma("unroll")
+        for (int u = 0; u < 12; u++) {
+            const int e = t2 + u * n2, a = e >> 5, f = e & 31;
+            if (e < 80 * 32) tw[a * LDW + f] = (f < nf) ? buf[u] * sinv[f0 + f] : 0.0;
+        }
+        CERB_BAR_SYNC(1, n2);
+        PH_MARK_T(38, 32);
+        if (f0 + 32 < nF) fetch(f0 + 32);
+        schur_tile_w(wq, tw, acc, lane);
+        CERB_BAR_SYNC(1, n2);
+        PH_MARK_T(39, 32);
+    }
+    schur_scatter_w(wq, s, acc, lane);
+    PH_MARK_T(7, 32);
+}
+// T = L^-1 Hyx (row a of Hxy in place; row 79: the y part of the rhs), rows on threads 32..111: block f of the forward substitution
+// starts as soon as warp 0 has published the factor of block f, so that the substitution finishes right behind the chain instead of after it
+CERB_D void forward_subst(Smem &s, const int *chain_done, int t2) {
+    if (t2 <= NX) {
+        double *row = (t2 < NX) ? s.Hxy + t2 * NY : s.yv + NX;
+        double tp[NYB];
+        _Pragma("unroll")
+        for (int k = 0; k < NYB; k++) tp[k] = 0.0;
+        _Pragma("unroll 1")
+        for (int f = 0; f < NFR; f++) {
+            while (CERB_LD_ACQUIRE_S32(chain_done) <= f) { CERB_SPIN_PAUSE(); }
+            __threadfence_block();
+            const double *L = s.Ad + f * HBLK, *idg = s.idg + NYB * f;
+            double *t = row + NYB * f;
+            double tc[NYB];
+            _Pragma("unroll")
+            for (int r = 0; r < NYB; r++) tc[r] = t[r];
+            if (f > 0) {
+                const double *M = s.Bo + (f - 1) * HBLK;
+                _Pragma("unroll")
+                for (int r = 0; r < NYB; r++) { double acc = 0.0; _Pragma("unroll") for (int q = 0; q < NYB; q++) acc += M[r * NYB + q] * tp[q]; tc[r] -= acc; }
+            }
+            _Pragma("unroll")
+            for (int c = 0; c < NYB; c++) {             // right-looking: the dependency chain is 13 (multiply, update) steps
+                tc[c] *= idg[c];
+                _Pragma("unroll")
+                for (int r = c + 1; r < NYB; r++) tc[r] -= L[r * NYB + c] * tc[c];
+            }
+            _Pragma("unroll")
+            for (int r = 0; r < NYB; r++) { t[r] = tc[r]; tp[r] = tc[r]; }
+        }
+    }
+}
+// dense Cholesky of the 79 x 79 lower triangle, rhs carried as row 79 (z = L^-1 rhs), blocked by panels of 8,
+// with look-ahead: (a) warp 0 factors a diagonal block in registers (pivots / column entries exchanged by shuffles),
+// (b) one thread per row below solves its 8 panel entries against L_kk, (c) the trailing lower triangle is updated
+// block by block on the fp64 tensor cores (A_ij -= L_ik L_jk^T, K = 8) -- warp 0 takes only the block that becomes
+// the next diagonal block and factors it right away, while warps 1..7 update the rest.  Two barriers per panel; the
+// serial column sweeps of the diagonal blocks (the critical path) overlap with the trailing updates.
+CERB_D void panel_cholesky(Smem &s, int tid) {
+    const int wq = tid >> 5, lane = tid & 31;
+    auto factor_diag = [&](int c0, int nb, double *Lkk) {      // warp 0: L_kk of the nb x nb block at (c0, c0); Lkk[64..72) = 1 / diag
+        const bool act = lane < nb;
+        const int r = act ? lane : 0;
+        double a[8];
+        _Pragma("unroll")
+        for (int c = 0; c < 8; c++) a[c] = (c < nb && c <= r) ? s.Hxx[(c0 + r) * NX + c0 + c] : 0.0;
+        double myinv = 1.0;
+        _Pragma("unroll")
+        for (int j = 0; j < 8; j++) {
+            double d = __shfl_sync(0xffffffffu, a[j], j);
+            if (j < nb && !(d > 0.0)) { if (lane == 0) s.sca[S_OK] = 0; }
+            if (!(d > 0.0)) d = 1.0;
+            const double inv = rsqrt(d);
+            if (lane == j) myinv = inv;
+            const double l = (lane == j) ? d * inv : a[j] * inv;
+            a[j] = l;
+            _Pragma("unroll")
+            for (int k = j + 1; k < 8; k++) { const double lk = __shfl_sync(0xffffffffu, l, k); a[k] -= l * lk; }
+        }
+        if (act) {
+            _Pragma("unroll")
+            for (int c = 0; c < 8; c++) if (c <= r) { s.Hxx[(c0 + r) * NX + c0 + c] = a[c]; Lkk[r * 8 + c] = a[c]; }
+            Lkk[64 + r] = myinv; s.idx[c0 + r] = myinv;
+        }
+    };
+    auto trailing_block = [&](int c0, int b0, int b) {          // block b = (bi, bj), bj <= bi, of the rows / columns from 8 b0 on
+        int bi = 0, idx = b;
+        while (idx > bi) { idx -= bi + 1; bi++; }
+        const int ri = 8 * (b0 + bi) + (lane >> 2), rj = 8 * (b0 + idx) + (lane >> 2);
+        double a0 = 0.0, a1 = 0.0;
+        for (int ks = 0; ks < 2; ks++) {
+            const int cc = c0 + 4 * ks + (lane & 3);
+            const double av = (ri < NX) ? s.Hxx[ri * NX + cc] : (ri == NX ? s.yv[cc] : 0.0);
+            const double bv = (rj < NX) ? s.Hxx[rj * NX + cc] : 0.0;
+            CERB_DMMA(a0, a1, av, bv, a0, a1);
+        }
+        const int cj = 8 * (b0 + idx) + 2 * (lane & 3);
+        if (ri < NX) {
+            if (cj <= ri && cj < NX) s.Hxx[ri * NX + cj] -= a0;
+            if (cj + 1 <= ri && cj + 1 < NX) s.Hxx[ri * NX + cj + 1] -= a1;
+        } else if (ri == NX) {
+            if (cj < NX) s.yv[cj] -= a0;
+            if (cj + 1 < NX) s.yv[cj + 1] -= a1;
+        }
+    };
+    if (wq == 0) factor_diag(0, 8, s.red);
+    __syncthreads();
+    int pk = 0;
+    for (int c0 = 0; c0 < NX; c0 += 8, pk ^= 1) {
+        const int nb = (NX - c0) < 8 ? (NX - c0) : 8, c1 = c0 + nb;
+        const double *Lkk = s.red + 80 * pk;            // factored diagonal block of this panel (+ inverse diagonal at [64..72))
+        // (b) rows c1 .. NX (row NX = rhs, kept in yv)
+        if (tid <= NX - c1) {
+            const int i = c1 + tid;
+            double *row = (i < NX) ? s.Hxx + i * NX + c0 : s.yv + c0;
+            double t[8];
+            _Pragma("unroll")
+            for (int c = 0; c < 8; c++) t[c] = (c < nb) ? row[c] : 0.0;
+            _Pragma("unroll")
+            for (int c = 0; c < 8; c++) {
+                if (c < nb) {
+                    t[c] *= Lkk[64 + c];
+                    _Pragma("unroll")
+                    for (int c2 = c + 1; c2 < 8; c2++) if (c2 < nb) t[c2] -= t[c] * Lkk[c2 * 8 + c];
+                }
+            }
+            _Pragma("unroll")
+            for (int c = 0; c < 8; c++) if (c < nb) row[c] = t[c];
+        }
+        __syncthreads();
+        if (c1 >= NX) break;
+        // (c) trailing update of rows / columns c1 .. NX (row NX = rhs) + look-ahead factorisation of the next diagonal block
+        {
+            const int b0 = c1 >> 3, nbt = 10 - b0;               // block rows b0 .. 9
+            const int nblk = nbt * (nbt + 1) / 2;
+            if (wq == 0) {
+                trailing_block(c0, b0, 0);
+                __syncwarp();
+                factor_diag(c1, (NX - c1) < 8 ? (NX - c1) : 8, s.red + 80 * (pk ^ 1));
+            } else {
+                for (int b = wq; b < nblk; b += 7) trailing_block(c0, b0, b);
+            }
+        }
+        __syncthreads();
+    }
+}
+// back substitutions for y_x, y_y and the inverse depths; the prior image's Hxx part is prefetched as soon as the factor of Hxx is dead
+CERB_D void back_substitution(const SolveParams &P, Smem &s, const Win &c, PriorCopy &pc, double mu, int &gn_attempts, int tid PH_ARG) {
+    // L^T y_x = z by warp 0: lane holds y[lane], y[lane + 32], y[lane + 64] in registers;
+    // branch-free steps (selects), the L entries of the next step are loaded before the current shuffle completes
+    if (tid < 32) {
+        double y0 = s.yv[tid], y1 = s.yv[32 + tid], y2 = (64 + tid < NX) ? s.yv[64 + tid] : 0.0;
+        _Pragma("unroll 1")
+        for (int k = NX - 1; k >= 0; k--) {
+            const double *Lk = s.Hxx + k * NX;
+            const double ik = s.idx[k];
+            const double l0 = (tid < k) ? Lk[tid] : 0.0, l1 = (32 + tid < k) ? Lk[32 + tid] : 0.0, l2 = (64 + tid < k) ? Lk[64 + tid] : 0.0;
+            const double src = (k >= 64) ? y2 : (k >= 32 ? y1 : y0);
+            const double yk = __shfl_sync(0xffffffffu, src, k & 31) * ik;
+            y0 = (tid == k) ? yk : y0 - l0 * yk;
+            y1 = (32 + tid == k) ? yk : y1 - l1 * yk;
+            y2 = (64 + tid == k) ? yk : y2 - l2 * yk;
+        }
+        s.yv[tid] = y0; s.yv[32 + tid] = y1; if (64 + tid < NX) s.yv[64 + tid] = y2;
+    }
+    __syncthreads();
+    if (c.has_prior) {                                                                         // the factor of Hxx is dead from here on
+        if (c.bulk_ok) { if (tid == 0) CERB_BULK_G2S(s.Hxx, c.ws.pimg, PIMG_HXY * 8, &s.mbar[0]); }
+        else copy_g2s_async(s.Hxx, c.ws.pimg, HXX_SZ, tid);
+        pc.hxx_prefetched = true;
+    }
+    PH_MARK(11);
+    // y part: u = gy' - T^T y_x, then L^T y_y = u blockwise (warp 0)
+    for (int q = tid; q < NY; q += SOLVE_THREADS) { double t = 0.0; for (int a = 0; a < NX; a++) t += s.Hxy[a * NY + q] * s.yv[a]; s.yv[NX + q] -= t; }
+    __syncthreads();
+    if (tid < 32) {      // lane r holds component r of the current block; one shuffle per substitution step
+        const int r = tid < NYB ? tid : 0;
+        double yn[NYB];                                  // solved block f + 1 (all lanes)
+        _Pragma("unroll")
+        for (int k = 0; k < NYB; k++) yn[k] = 0.0;
+        _Pragma("unroll 1")
+        for (int f = NFR - 1; f >= 0; f--) {
+            const double *L = s.Ad + f * HBLK;
+            double u = s.yv[NX + NYB * f + r];
+            if (f < NFR - 1) {
+                const double *M = s.Bo + f * HBLK;
+                double t = 0.0;
+                _Pragma("unroll")
+                for (int k = 0; k < NYB; k++) t += M[k * NYB + r] * yn[k];
+                u -= t;
+            }
+            double lc[NYB], ig[NYB];                          // column r of L^T and the inverse pivots: loaded before the chain
+            _Pragma("unroll")
+            for (int k = 0; k < NYB; k++) { lc[k] = (tid < k) ? L[k * NYB + r] : 0.0; ig[k] = s.idg[NYB * f + k]; }
+            _Pragma("unroll")
+            for (int k = NYB - 1; k >= 0; k--) {
+                const double yk = __shfl_sync(0xffffffffu, u, k) * ig[k];
+                yn[k] = yk;
+                u = (tid == k) ? yk : u - lc[k] * yk;
+            }
+            if (tid < NYB) s.yv[NX + NYB * f + tid] = u;
+        }
+    }
+    __syncthreads();
+    PH_MARK(12);
+    // inverse depths: y_l = (gl - w^T y_x) / (h + mu D^2) ; validity
+    double bad = 0.0;
+    for (int f = tid; f < c.nF; f += SOLVE_THREADS) {
+        double t = c.ws.gl[f];
+        for (int a = 0; a < NX; a++) t -= c.ws.W[(size_t)a * c.ws.F + f] * s.yv[a];
+        const double y = t / (c.ws.hh[f] + mu * c.ws.Dl[f] * c.ws.Dl[f]);
+        c.ws.gnl[f] = y;
+        if (!(fabs(y) < 1e300)) bad = 1.0;
+    }
+    for (int k = tid; k < NR; k += SOLVE_THREADS) if (!(fabs(s.yv[k]) < 1e300)) bad = 1.0;
+    if (bad != 0.0) s.sca[S_OK] = 0;          // benign race: every writer stores 0
+    if (gn_attempts < P.test_fail_factorizations) s.sca[S_OK] = 0;      // fault injection of the parity tests (0 in production)
+    gn_attempts++;
+    __syncthreads();
+    PH_MARK(13);
+}
+// Gauss-Newton step (H~ + mu D^2) y = g~ -> gn = -D y (s.gn, gnl) and its norms; S_OK = 0 if it failed
+CERB_D void gauss_newton_step(const SolveParams &P, Smem &s, const Win &c, PriorCopy &pc, int &gn_attempts, int tid PH_ARG) {
+    const int nF = c.nF;
+    const double mu = s.sca[S_MU];
+    // rhs: yv[0..NR) = g~ ; regularise the diagonal of Hyy (that of Hxx: warps 1..7, after their share of v^T H v)
+    for (int k = tid; k < NR; k += SOLVE_THREADS) {
+        s.yv[k] = s.g[k];
+        if (k >= NX) s.Ad[((k - NX) / NYB) * HBLK + ((k - NX) % NYB) * (NYB + 1)] += mu * s.D[k] * s.D[k];
+    }
+    int *chain_done = s.ti + TI_CHAIN_DONE;
+    if (tid == 0) *chain_done = 0;
+    __syncthreads();
+    if (tid < 32) chain_cholesky(s, chain_done, tid PH_FWD);
+    else { lambda_schur(s, c, mu, tid PH_FWD); forward_subst(s, chain_done, tid - 32); }
+    __syncthreads();
+    if (tid == 0) {
+        double vhv = s.sca[S_VHV];
+        for (int k = 0; k < 7; k++) vhv += s.lin[k];
+        s.sca[S_ALPHA] = s.sca[S_GNORM2] / vhv;
+    }
+    PH_MARK(5);
+    __syncthreads();
+    PH_MARK(8);
+    // S' = S - T T^T (lower), rhs'_x = rhs_x - T gy' : Gram matrix of the 79 x 143 matrix [T; gy'^T] on the
+    // fp64 tensor cores, K = 143 padded to 144; block rectangles per warp, see ttt_warp
+    ttt_warp_w(tid >> 5, s, tid & 31);
+    __syncthreads();
+    PH_MARK(9);
+    panel_cholesky(s, tid);
+    PH_MARK(10);
+    back_substitution(P, s, c, pc, mu, gn_attempts, tid PH_FWD);
+    if (s.sca[S_OK] != 0.0) {      // gauss_newton_step = -D * y ; norms for the dogleg
+        double part3[2] = {0.0, 0.0};    // ||gn||^2, gh . gn
+        for (int k = tid; k < NR; k += SOLVE_THREADS) { const double v = -s.D[k] * s.yv[k]; s.gn[k] = v; part3[0] += v * v; part3[1] += s.gh[k] * v; }
+        for (int f = tid; f < nF; f += SOLVE_THREADS) { const double v = -c.ws.Dl[f] * c.ws.gnl[f]; c.ws.gnl[f] = v; part3[0] += v * v; part3[1] += c.ws.ghl[f] * v; }
+        double tot3[2];
+        block_sum<2>(part3, s.red, tot3, tid);
+        if (tid == 0) { s.sca[S_GNNORM2] = tot3[0]; s.sca[S_GDOTGN] = tot3[1]; }
+        __syncthreads();
+    }
+}
+// ComputeTraditionalDoglegStep: S_P, S_Q (step = (p gh + q gn) / D), its norm and the model cost change
+CERB_D void dogleg_step(double *sca, int tid) {
+    if (tid == 0) {
+        const double radius = sca[S_RADIUS], alpha = sca[S_ALPHA];
+        const double gradient_norm = sqrt(sca[S_GNORM2]), gauss_newton_norm = sqrt(sca[S_GNNORM2]);
+        double p, q, nrm;
+        if (gauss_newton_norm <= radius) { p = 0.0; q = 1.0; nrm = gauss_newton_norm; }
+        else if (gradient_norm * alpha >= radius) { p = -(radius / gradient_norm); q = 0.0; nrm = radius; }
+        else {
+            const double b_dot_a = -alpha * sca[S_GDOTGN];
+            const double a_squared_norm = (alpha * gradient_norm) * (alpha * gradient_norm);
+            const double b_minus_a_squared_norm = a_squared_norm - 2 * b_dot_a + gauss_newton_norm * gauss_newton_norm;
+            const double c = b_dot_a - a_squared_norm;
+            const double d = sqrt(c * c + b_minus_a_squared_norm * (radius * radius - a_squared_norm));
+            const double beta = (c <= 0) ? (d - c) / b_minus_a_squared_norm : (radius * radius - a_squared_norm) / (d + c);
+            p = -alpha * (1.0 - beta); q = beta;
+            nrm = sqrt(p * p * sca[S_GNORM2] + 2 * p * q * sca[S_GDOTGN] + q * q * sca[S_GNNORM2]);
+        }
+        sca[S_P] = p; sca[S_Q] = q; sca[S_DLNORM] = nrm;
+        // model_cost_change = -(step^T g~ + 0.5 step^T H~ step) with step = (p gh + q gn) / D, using
+        // H~ (gn/D) = -(g~ + mu D gn)  (the Gauss-Newton equations):
+        const double mu = sca[S_MU], g2 = sca[S_GNORM2], gg = sca[S_GDOTGN], n2 = sca[S_GNNORM2];
+        const double sTg = p * g2 + q * gg;
+        const double sHs = p * p * (g2 / alpha) - 2.0 * p * q * (g2 + mu * gg) + q * q * (-gg - mu * n2);
+        sca[S_MODEL] = -(sTg + 0.5 * sHs);
+    }
+    __syncthreads();
+}
+// HandleInvalidStep (LINEAR_SOLVER_FAILURE or a step without model decrease; the failed factorisation overwrote H, so the caller
+// re-linearises at the same point); true: the minimizer stops
+CERB_D bool handle_invalid_step(double *sca, int tid) {
+    if (tid == 0) {
+        sca[S_INVALID] += 1;
+        if (sca[S_INVALID] >= 5) { sca[S_DONE] = 1; sca[S_TERM] = 2; }
+        sca[S_MU] *= 10.0; sca[S_REUSE] = 0;      // StepIsInvalid
+    }
+    __syncthreads();
+    return sca[S_DONE] != 0.0;
+}
+// candidate point x [+] delta, lam + dlam, its cost (S_CCOST) and ||delta|| (S_STEPNORM).  Speculative linearisation: if the previous step of
+// this window was accepted, the candidate is linearised right away -- its cost is the candidate cost, and when the step is accepted (the common
+// case) the linearisation of the next iteration is already there, so the separate cost-only pass is saved.  A rejected step leaves H / g / W at
+// the candidate, which is harmless: the re-use path of the dogleg needs none of them.  Not done in the last allowed iteration (never needed).
+CERB_D void evaluate_candidate(const SolveParams &P, Smem &s, const Win &c, PriorCopy &pc, bool speculate, int tid PH_ARG) {
+    const int nF = c.nF;
+    double *sca = s.sca, *stl = c.ws.stl, *lamc = c.ws.lamc;
+    {   // delta = ((p gh + q gn) / D) * jacobi_scale
+        const double p = sca[S_P], q = sca[S_Q];
+        for (int k = tid; k < NR; k += SOLVE_THREADS) s.stp[k] = (p * s.gh[k] + q * s.gn[k]) / s.D[k] * s.sc[k];
+        for (int f = tid; f < nF; f += SOLVE_THREADS) stl[f] = (p * c.ws.ghl[f] + q * c.ws.gnl[f]) / c.ws.Dl[f] * c.ws.sl[f];
+    }
+    __syncthreads();
+    PH_MARK(14);
+    apply_plus(s, s.stp, c.lam, stl, lamc, nF, c.ex_open, c.td_open, tid);
+    double part[2];
+    PH_MARK(15);
+    if (speculate) { linearize(P, s, c, pc, s.xc, lamc, false, tid PH_FWD); part[0] = 0.0; }
+    else {
+        load_geometry(s.xc, s, tid);
+        part[0] = vision_cost(P, c.w, s.xc, lamc, tid);
+        PH_MARK(16);
+        part[0] += inertial_cost(P, c.w, s.xc, tid);
+    }
+    PH_MARK(17);
+    part[1] = ambient_sq(s.xs, s.xc, c.lam, lamc, nF, c.ex_open, c.lb_open, c.td_open, tid);
+    double tot[2];
+    block_sum<2>(part, s.red, tot, tid);
+    if (tid == 0) {
+        double cc = speculate ? sca[S_LCOST] : tot[0];
+        if (!(cc == cc) || fabs(cc) > 1e300) cc = 1.7976931348623157e308;
+        sca[S_CCOST] = cc; sca[S_STEPNORM] = sqrt(tot[1]);
+    }
+    __syncthreads();
+}
+// tolerances, then StepAccepted (S_OK = 2) / StepRejected; true: the minimizer stops
+CERB_D bool accept_or_reject(const SolveParams &P, double *sca, int tid) {
+    if (tid == 0) {
+        const double x_cost = sca[S_XCOST], cand = sca[S_CCOST];
+        if (sca[S_STEPNORM] <= P.ptol * (sca[S_XNORM] + P.ptol)) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
+        else if (fabs(x_cost - cand) <= P.ftol * x_cost) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
+        else {
+            const double rel = (x_cost - cand) / sca[S_MODEL];
+            if (rel > P.min_rel_dec) {            // StepAccepted
+                if (rel < 0.25) sca[S_RADIUS] *= 0.5;
+                if (rel > 0.75) sca[S_RADIUS] = fmax(sca[S_RADIUS], 3.0 * sca[S_DLNORM]);
+                sca[S_MU] = fmax(1e-8, 2.0 * sca[S_MU] / 10.0);
+                sca[S_REUSE] = 0; sca[S_NSUCC] += 1; sca[S_OK] = 2;     // 2 == accepted marker
+                sca[S_XCOST] = cand;                                   // x_cost of the new point (re-evaluated by the next linearisation, if any)
+            } else {                              // StepRejected
+                sca[S_RADIUS] *= 0.5; sca[S_REUSE] = 1; sca[S_OK] = 1;
+            }
+        }
+    }
+    __syncthreads();
+    return sca[S_DONE] != 0.0;
 }
 
 // ---- the kernel -----------------------------------------------------------------------------------------------
@@ -942,715 +1609,78 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, CERB_SOLVE_MIN_BLOCKS) vilo_so
     CERB_DYN_SMEM(double, smem_base);
     Smem s; smem_carve(smem_base, s);
     const int tid = threadIdx.x;
-    const int F = P.maxF;
-    double *ws = P.ws + (size_t)blockIdx.x * P.ws_stride;
-    double *W = ws + ws_W(F);
-    double *hh = ws + ws_vecs(F), *gl = hh + F, *sl = gl + F, *Dl = sl + F, *ghl = Dl + F, *gnl = ghl + F, *stl = gnl + F, *lamc = stl + F;
-    int *chunks = reinterpret_cast<int *>(ws + ws_chunks(F));          // [0] n, [1..n] chunk starts, [n + 1] nF
-    double *pimg = ws + ws_prior(F);                                   // prior Hessian image, built once per window
+    const CtaWs ws = ws_carve(P);
     double *sca = s.sca;
-    // scalar slots
-    enum { S_RADIUS = 0, S_MU, S_REUSE, S_XCOST, S_CCOST, S_ALPHA, S_GNORM2, S_GNNORM2, S_GDOTGN, S_MODEL, S_STEPNORM, S_XNORM, S_DLNORM,
-           S_OK, S_DONE, S_TERM, S_ITER, S_NSUCC, S_INVALID, S_GMAX, S_INIT_COST, S_P, S_Q, S_VHV, S_LCOST, S_LNORM, S_LGMAX };
-
     PH_DECL();
-    unsigned par0 = 0, par1 = 0;                                          // phase parities of the two bulk-copy mbarriers (uniform over the CTA)
+    PriorCopy pc = {0, 0, false};
     if (tid == 0) { CERB_MBAR_INIT(&s.mbar[0]); CERB_MBAR_INIT(&s.mbar[1]); }
-    if (tid < 32) {
-        // Scatter plan of the 40 x 40 IMU-leg Gram matrix (inertial_linearize): lane `tid` holds, for block q = (mi, ni) and
-        // e = 0, 1, the entry (la, lb) = (8 mi + lane / 4, 8 ni + 2 (lane % 4) + e).  Its destination in Hxx / Hxy / Hyy / g is
-        // affine in the factor index i, so the plan stores two ints: offset(i = 0) and stride | (mirror delta + 256) << 12 (in doubles
-        // from the start of shared memory; the mirror is the transposed entry of a diagonal Hyy block).  Entries without a destination
-        // point at a per-lane dummy slot (idg[32 warp + lane], never read) with stride 0.
-        int *plan = reinterpret_cast<int *>(ws + ws_imuplan(F));
-        int q = 0;
-        for (int mi = 0; mi < 5; mi++)
-            for (int ni = mi; ni < 5; ni++, q++)
-                for (int e = 0; e < 2; e++) {
-                    const int la = 8 * mi + (tid >> 2), lb = 8 * ni + 2 * (tid & 3) + e;
-                    int px = (int)(s.idg - smem_base) + tid, py = 256 << 12;         // default: dummy slot of this lane (idg is idle during a linearisation; each IMU warp adds 32 x its index), stride 0, delta 0
-                    if (la <= lb && lb <= 38 && la != 38) {
-                        double *p0[2], *p1[2];
-                        for (int i = 0; i < 2; i++) {
-                            const int da = imu_col_dest(i, la);
-                            if (lb == 38) { p0[i] = da >= 0 ? s.g + da : s.g + NX + (-da - 1); p1[i] = nullptr; }
-                            else scatter_addr(s, da, imu_col_dest(i, lb), &p0[i], &p1[i]);
-                        }
-                        px = (int)(p0[0] - smem_base);
-                        py = (int)(p0[1] - p0[0]) | (((p1[0] ? (int)(p1[0] - p0[0]) : 0) + 256) << 12);
-                    }
-                    plan[(2 * (q * 2 + e)) * 32 + tid] = px; plan[(2 * (q * 2 + e) + 1) * 32 + tid] = py;
-                }
-    }
+    build_imu_plan(s, smem_base, ws.imu_plan, tid);
     __syncthreads();
     for (int w = blockIdx.x; w < P.n_windows; w += gridDim.x) {
-        const int nF = P.n_features[w];
-        const bool ex_open = (P.flags[w] & 1) != 0;
-        const bool lb_open = P.optimize_leg_bias && (P.flags[w] & 4) == 0;
-        const bool td_open = (P.flags[w] & 2) != 0;
-        double *lam = P.lam + (size_t)w * F;
-        if (tid == 0) {      // feature chunks: <= 64 consecutive tracks with the same anchor frame
-            int n = 0, c0 = 0;
-            while (c0 < nF) {
-                chunks[1 + n] = c0;
-                const int a = P.feat_start[(size_t)w * F + c0];
-                int e = c0 + 1;
-                while (e < nF && e < c0 + 64 && P.feat_start[(size_t)w * F + e] == a) e++;
-                if (n < 15) { s.ti[97 + 2 * n] = c0; s.ti[98 + 2 * n] = ((e - c0) << 8) | a; }      // the first 15 chunks are also cached in shared memory
-                n++; c0 = e;
-            }
-            chunks[1 + n] = nF; chunks[0] = n; s.ti[96] = n;
-        }
-        // prior Hessian image (J0^T J0 scattered into the layout of Hxx | Hxy | Ad | Bo): constant during the solve, every
-        // linearisation starts from it instead of from zero.  s.ti keeps the column -> destination map of the prior.
-        const bool has_prior = build_prior_image(P, s, w, pimg, tid);
-        if (tid == 0) s.ti[131] = 0;                                    // all IMU-leg factors (the marginalization kernel restricts them)
+        Win c; c.w = w; c.nF = P.n_features[w]; c.ws = ws; c.lam = P.lam + (size_t)w * ws.F;
+        c.ex_open = (P.flags[w] & 1) != 0; c.lb_open = P.optimize_leg_bias && (P.flags[w] & 4) == 0; c.td_open = (P.flags[w] & 2) != 0;
+        if (tid == 0) build_chunks(P.feat_start + (size_t)w * ws.F, s, ws.chunks, c.nF);
+        c.has_prior = build_prior_image(P, s, w, ws.pimg, tid);
+        if (tid == 0) s.ti[TI_IMU_MASK] = 0;                             // all IMU-leg factors (the marginalization kernel restricts them)
         for (int k = tid; k < ST_STRIDE; k += SOLVE_THREADS) s.xs[k] = (k < ST_SIZE) ? P.state[(size_t)w * ST_STRIDE + k] : 0.0;
         if (tid == 0) {
             sca[S_RADIUS] = P.radius0; sca[S_MU] = P.test_initial_mu > 0.0 ? P.test_initial_mu : 1e-8; sca[S_REUSE] = 0; sca[S_DONE] = 0; sca[S_TERM] = 1; sca[S_ITER] = 0; sca[S_NSUCC] = 0;
             sca[S_INVALID] = 0; sca[S_DLNORM] = 0;
         }
         __syncthreads();
-        const bool bulk_ok = (reinterpret_cast<uintptr_t>(pimg) & 15) == 0 && !P.no_bulk_copy;          // TMA bulk copies need 16-byte aligned sources (max_features even)
-        bool need_linearize = true, hxx_prefetched = false, last_accepted = true;
+        c.bulk_ok = (reinterpret_cast<uintptr_t>(ws.pimg) & 15) == 0 && !P.no_bulk_copy;          // TMA bulk copies need 16-byte aligned sources (max_features even)
+        pc.hxx_prefetched = false;
+        bool need_linearize = true, last_accepted = true;
         int iteration = 0, gn_attempts = 0;
-
-        // ---- linearisation at (xl, laml): H, g (Jacobi scaled), W, hh, gl; results S_LCOST (cost), S_LNORM (||x||), S_LGMAX (max |g|) --------
-        auto linearize = [&](const double *xl, const double *laml, bool first) {
-                // start from the prior Hessian image; its Hxx part was prefetched asynchronously when the previous factorisation of
-                // Hxx had been consumed (the copy overlapped with the rest of that iteration), except for the first linearisation
-                if (!has_prior) { for (int k = tid; k < HXX_SZ; k += SOLVE_THREADS) s.Hxx[k] = 0.0; }
-                else if (bulk_ok) {
-                    if (!hxx_prefetched) { __syncthreads(); if (tid == 0) CERB_BULK_G2S(s.Hxx, pimg, PIMG_HXY * 8, &s.mbar[0]); }
-                    CERB_MBAR_WAIT(&s.mbar[0], par0); par0 ^= 1;
-                } else { if (!hxx_prefetched) copy_g2s_async(s.Hxx, pimg, HXX_SZ, tid); CERB_CP_ASYNC_WAIT(); }
-                hxx_prefetched = false;
-                for (int k = tid; k < NRP; k += SOLVE_THREADS) s.g[k] = 0.0;
-                load_geometry(xl, s, tid);
-                double part[2];
-                PH_MARK(0);
-                part[0] = vision_linearize(P, w, xl, laml, W, hh, gl, sl, !first, chunks, tid);
-                if (has_prior && bulk_ok) {                                                                  // Hxy | Ad | Bo (contiguous; the tile aliased them):
-                    if (tid == 0) CERB_BULK_G2S(s.Hxy, pimg + PIMG_HXY, PIMG_REST * 8, &s.mbar[1]);            // one bulk copy (vision_linearize ended with a barrier)
-                    CERB_MBAR_WAIT(&s.mbar[1], par1); par1 ^= 1;
-                } else if (has_prior) copy_g2s_async(s.Hxy, pimg + PIMG_HXY, PIMG_REST, tid);                 // completed inside inertial_linearize
-                else for (int k = tid; k < PIMG_REST; k += SOLVE_THREADS) s.Hxy[k] = 0.0;
-                __syncthreads();
-                PH_MARK(1);
-                part[0] += inertial_linearize(P, w, xl, tid);
-                PH_MARK(2);
-                part[1] = ambient_sq(xl, nullptr, laml, nullptr, nF, ex_open, lb_open, td_open, tid);
-                double tot[2];
-                block_sum<2>(part, s.red, tot, tid);
-                if (tid == 0) { sca[S_LCOST] = tot[0]; sca[S_LNORM] = sqrt(tot[1]); }
-                // (Hxx holds its upper triangle; it is mirrored and scaled in one row-wise pass below)
-                // gradient max norm over active dims (unscaled), Jacobi scale at the first linearisation
-                if (first) {
-                    for (int k = tid; k < NR; k += SOLVE_THREADS) {
-                        double d;
-                        bool active = true;
-                        if (k < NX) { d = s.Hxx[k * NX + k]; if (k >= 66 && k < X_TD && !ex_open) active = false; if (k == X_TD && !td_open) active = false; }
-                        else { const int yk = k - NX, f = yk / NYB, c = yk % NYB; d = s.Ad[f * 169 + c * NYB + c]; if (c >= 9 && !lb_open) active = false; }
-                        s.sc[k] = active ? 1.0 / (1.0 + sqrt(d)) : 0.0;
-                    }
-                    for (int f = tid; f < nF; f += SOLVE_THREADS) sl[f] = 1.0 / (1.0 + sqrt(hh[f]));
-                }
-                __syncthreads();
-                if (P.dbg && w == P.dbg_window && first) {      // parity probe, ABI order
-                    for (int k = tid; k < NR; k += SOLVE_THREADS) {
-                        int dst; double d;
-                        if (k < NX) { dst = k < X_TD ? k : 221; d = s.Hxx[k * NX + k]; }      // ABI order: td after the leg biases
-                        else { const int yk = k - NX, f = yk / NYB, c = yk % NYB; dst = c < 9 ? 78 + 9 * f + c : 177 + 4 * f + (c - 9); d = s.Ad[f * 169 + c * NYB + c]; }
-                        const bool act = s.sc[k] != 0.0;
-                        P.dbg[1 + dst] = act ? s.g[k] : 0.0; P.dbg[1 + NR + F + dst] = act ? d : 0.0;
-                    }
-                    for (int f = tid; f < nF; f += SOLVE_THREADS) { P.dbg[1 + NR + f] = gl[f]; P.dbg[1 + NR + F + NR + f] = hh[f]; }
-                    if (tid == 0) P.dbg[0] = sca[S_LCOST];
-                }
-                double gm = 0.0;
-                for (int k = tid; k < NR; k += SOLVE_THREADS) if (s.sc[k] != 0.0) gm = fmax(gm, fabs(s.g[k]));
-                for (int f = tid; f < nF; f += SOLVE_THREADS) gm = fmax(gm, fabs(!first ? gl[f] / sl[f] : gl[f]));   // unscaled gradient
-                for (int o = 16; o > 0; o >>= 1) gm = fmax(gm, __shfl_sync(0xffffffffu, gm, (tid + o) & 31));
-                if ((tid & 31) == 0) s.red[tid >> 5] = gm;
-                __syncthreads();
-                if (tid == 0) { double m8 = s.red[0]; for (int k = 1; k < SOLVE_THREADS / 32; k++) m8 = fmax(m8, s.red[k]); sca[S_LGMAX] = m8; }
-                // apply the Jacobi scaling: H~ = S H S, g~ = S g, w~_f = s_f S_x w_f, h~ = s_f^2 h, gl~ = s_f gl.  Row-wise (a warp per
-                // row: no index divisions); the Hxx pass also mirrors the upper triangle into the lower one.
-                for (int a = tid >> 5; a < NX; a += SOLVE_THREADS / 32) {
-                    const double sa = s.sc[a];
-                    for (int b = a + (tid & 31); b < NX; b += 32) { const double v = s.Hxx[a * NX + b] * (sa * s.sc[b]); s.Hxx[a * NX + b] = v; s.Hxx[b * NX + a] = v; }
-                    for (int q = tid & 31; q < NY; q += 32) s.Hxy[a * NY + q] *= sa * s.sc[NX + q];
-                }
-                for (int k = tid; k < 1859; k += SOLVE_THREADS) { const int f = k / 169, a = (k % 169) / NYB, b = k % NYB; s.Ad[k] *= s.sc[NX + NYB * f + a] * s.sc[NX + NYB * f + b]; }
-                for (int k = tid; k < 1690; k += SOLVE_THREADS) { const int f = k / 169, a = (k % 169) / NYB, b = k % NYB; s.Bo[k] *= s.sc[NX + NYB * f + a] * s.sc[NX + NYB * (f + 1) + b]; }
-                for (int k = tid; k < NR; k += SOLVE_THREADS) s.g[k] *= s.sc[k];
-                if (first) {      // later linearisations write W, hh, gl pre-scaled
-                    for (int k = tid; k < NX * nF; k += SOLVE_THREADS) { const int a = k / nF, f = k % nF; W[(size_t)a * F + f] *= s.sc[a] * sl[f]; }
-                    for (int f = tid; f < nF; f += SOLVE_THREADS) { hh[f] *= sl[f] * sl[f]; gl[f] *= sl[f]; }
-                }
-                __syncthreads();
-        };
         while (true) {
-            // =============================== linearise at xs ===========================================
             // Ceres evaluates the Jacobian at every accepted point, but when that point is the last one allowed by max_num_iterations the
             // evaluation is never used: FinalizeIterationAndCheckIfMinimizerCanContinue tests the iteration limit before the gradient
             // tolerance, so termination, states and costs are decided already.  That last linearisation is skipped.
             if (need_linearize && (iteration < P.max_iters || iteration == 0)) {
-                linearize(s.xs, lam, iteration == 0);
+                linearize(P, s, c, pc, s.xs, c.lam, iteration == 0, tid PH_FWD);
                 if (tid == 0) { sca[S_XCOST] = sca[S_LCOST]; sca[S_XNORM] = sca[S_LNORM]; sca[S_GMAX] = sca[S_LGMAX]; if (iteration == 0) sca[S_INIT_COST] = sca[S_LCOST]; }
                 __syncthreads();
                 need_linearize = false;
                 PH_MARK(3);
             }
-            // =============================== FinalizeIterationAndCheckIfMinimizerCanContinue =============
-            if (tid == 0) {
-                if (iteration >= P.max_iters) { sca[S_DONE] = 1; sca[S_TERM] = 1; }
-                else if (sca[S_GMAX] <= P.gtol) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
-                else if (sca[S_RADIUS] <= P.min_radius) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
-                else if (!(sca[S_XCOST] == sca[S_XCOST]) || fabs(sca[S_XCOST]) > 1e300) { sca[S_DONE] = 1; sca[S_TERM] = 2; }
-            }
-            __syncthreads();
-            if (sca[S_DONE] != 0.0) break;
+            if (finalize_iteration(P, sca, iteration, tid)) break;
             iteration++;
-
-            // =============================== DoglegStrategy::ComputeStep ===================================
+            // DoglegStrategy::ComputeStep.  ComputeGaussNewtonStep retries INSIDE one ComputeStep (`while (mu_ < max_mu_)`, Ceres 1.14
+            // dogleg_strategy.cc): a failed factorisation / non-finite step multiplies mu by 10 and solves again at the same point -- no
+            // iteration and no invalid step is consumed; only when mu reaches max_mu (1.0) does the strategy report LINEAR_SOLVER_FAILURE.
+            // The factorisation here is in place, so a retry first rebuilds H / g at the same point.
             if (sca[S_REUSE] == 0.0) {
-              // DoglegStrategy::ComputeGaussNewtonStep retries INSIDE one ComputeStep (`while (mu_ < max_mu_)`, Ceres 1.14 dogleg_strategy.cc):
-              // a failed factorisation / non-finite step multiplies mu by 10 and solves again at the same point -- no iteration and no invalid
-              // step is consumed; only when mu reaches max_mu (1.0) does the strategy report LINEAR_SOLVER_FAILURE.  The factorisation here is
-              // in place, so a retry first rebuilds H / g at the same point.
-              for (;;) {
-                if (!(sca[S_MU] < 1.0)) {                 // while (mu_ < max_mu_) not entered: LINEAR_SOLVER_FAILURE without a solve
-                    __syncthreads();
-                    if (tid == 0) { sca[S_OK] = 0; sca[S_REUSE] = 1; }
-                    __syncthreads();
-                    break;
-                }
-                // diagonal, gradient / D, scaled gradient v (kept in s.stp: the Cauchy point's v^T H v is finished later, see below)
-                for (int k = tid; k < NR; k += SOLVE_THREADS) {
-                    const double d = (k < NX) ? s.Hxx[k * NX + k] : s.Ad[((k - NX) / NYB) * 169 + ((k - NX) % NYB) * (NYB + 1)];
-                    const double D = sqrt(fmin(fmax(d, 1e-6), 1e32));
-                    s.D[k] = D; s.gh[k] = s.g[k] / D; s.stp[k] = s.gh[k] / D;
-                }
-                for (int f = tid; f < nF; f += SOLVE_THREADS) { const double D = sqrt(fmin(fmax(hh[f], 1e-6), 1e32)); Dl[f] = D; ghl[f] = gl[f] / D; stl[f] = ghl[f] / D; }
-                __syncthreads();
-                // ||gh||^2 and the Hyy part of v^T H v (Hyy is about to be factored in place); the Hxx / Hxy / W parts are
-                // computed by warps 1..7 in the shadow of warp 0's chain factorisation
-                double part[2] = {0.0, 0.0};     // [0] v_y^T Hyy v_y  [1] ||gh||^2
-                for (int k = tid; k < 1859; k += SOLVE_THREADS) { const int f = k / 169, a = (k % 169) / NYB, b = k % NYB; part[0] += s.stp[NX + NYB * f + a] * s.Ad[k] * s.stp[NX + NYB * f + b]; }
-                for (int k = tid; k < 1690; k += SOLVE_THREADS) { const int f = k / 169, a = (k % 169) / NYB, b = k % NYB; part[0] += 2.0 * s.stp[NX + NYB * f + a] * s.Bo[k] * s.stp[NX + NYB * (f + 1) + b]; }
-                for (int f = tid; f < nF; f += SOLVE_THREADS) part[1] += ghl[f] * ghl[f];
-                for (int k = tid; k < NR; k += SOLVE_THREADS) part[1] += s.gh[k] * s.gh[k];
-                double tot[2];
-                block_sum<2>(part, s.red, tot, tid);
-                if (tid == 0) { sca[S_GNORM2] = tot[1]; sca[S_VHV] = tot[0]; sca[S_OK] = 1; }      // S_OK: a failure below is an invalid step: mu *= 10, re-linearise
-                PH_MARK(4);
-
-                // ---- Gauss-Newton step: (H~ + mu D^2) y = g~, retry with mu *= 10 on failure ----------------
-                {
-                    const double mu = sca[S_MU];
-                    // rhs: yv[0..NR) = g~ ; regularise the diagonal of Hyy (that of Hxx: warps 1..7, after their share of v^T H v)
-                    for (int k = tid; k < NR; k += SOLVE_THREADS) {
-                        s.yv[k] = s.g[k];
-                        if (k >= NX) s.Ad[((k - NX) / NYB) * 169 + ((k - NX) % NYB) * (NYB + 1)] += mu * s.D[k] * s.D[k];
-                    }
-                    int *chain_done = s.ti + 130;              // number of Hyy blocks whose factor (L_f, M_f) warp 0 has published
-                    if (tid == 0) *chain_done = 0;
-                    __syncthreads();
-                    if (tid < 32) {
-                        // ---- warp 0: block-bidiagonal Cholesky of Hyy: Ad[f] <- L_f (lower), Bo[f] <- M_f = B_f^T L_f^-T ----
-                        // Lane r owns row r of the 13 x 13 block in registers; the column sweep exchanges pivots and column
-                        // entries with shuffles (no shared-memory round trips on the dependency chain).
-                        const int lane = tid;
-                        const bool act = lane < NYB;
-                        const int r = act ? lane : 0;              // idle lanes shadow row 0 and never store
-                        double m[NYB];                             // row r of M_{f-1}
-                        _Pragma("unroll")
-                        for (int c = 0; c < NYB; c++) m[c] = 0.0;
-                        _Pragma("unroll 1")                        // keep the block body compact: it is re-used 11 times from the instruction cache
-                        for (int f = 0; f < NFR; f++) {
-                            double *A = s.Ad + f * 169;
-                            double a[NYB], invd[NYB], myinv = 1.0;
-                            _Pragma("unroll")
-                            for (int c = 0; c < NYB; c++) a[c] = A[r * NYB + c];
-                            if (f > 0) {
-                                const double *Mp = s.Bo + (f - 1) * 169;        // M[r][c], r: y_f index, c: y_{f-1} index
-                                _Pragma("unroll")
-                                for (int c = 0; c < NYB; c++) { double t = 0.0; _Pragma("unroll") for (int q = 0; q < NYB; q++) t += m[q] * Mp[c * NYB + q]; a[c] -= t; }
-                            }
-                            _Pragma("unroll")
-                            for (int j = 0; j < NYB; j++) {                     // right-looking column sweep
-                                double d = __shfl_sync(0xffffffffu, a[j], j);
-                                if (!(d > 0.0)) { if (lane == 0) sca[S_OK] = 0; d = 1.0; }
-                                const double inv = rsqrt(d);
-                                invd[j] = inv;
-                                if (lane == j) myinv = inv;
-                                const double l = (lane == j) ? d * inv : a[j] * inv;
-                                a[j] = l;
-                                // column j of L to all lanes through a double-buffered shared-memory line (1 store + 12 broadcast loads
-                                // instead of 12 two-instruction shuffles: the sweep is bound by the instruction issue of this one warp)
-                                double *colb = s.sca + 32 + 16 * (j & 1);
-                                if (act) colb[lane] = l;
-                                __syncwarp();
-                                _Pragma("unroll")
-                                for (int k = j + 1; k < NYB; k++) a[k] -= l * colb[k];
-                            }
-                            if (act) { _Pragma("unroll") for (int c = 0; c < NYB; c++) if (c <= r) A[r * NYB + c] = a[c]; s.idg[NYB * f + r] = myinv; }
-                            __syncwarp();
-                            if (f < NFR - 1) {
-                                double *B = s.Bo + f * 169;                     // in: B[k1][k2] = H(y_f[k1], y_{f+1}[k2]); out: M[r][c]
-                                double t[NYB];
-                                _Pragma("unroll")
-                                for (int c = 0; c < NYB; c++) t[c] = B[c * NYB + r];
-                                _Pragma("unroll")
-                                for (int c = 0; c < NYB; c++) {
-                                    m[c] = t[c] * invd[c];
-                                    _Pragma("unroll")
-                                    for (int c2 = c + 1; c2 < NYB; c2++) t[c2] -= m[c] * A[c2 * NYB + c];
-                                }
-                                __syncwarp();
-                                if (act) { _Pragma("unroll") for (int c = 0; c < NYB; c++) B[r * NYB + c] = m[c]; }
-                                __syncwarp();
-                            }
-                            __threadfence_block(); __syncwarp();
-                            if (lane == 0) CERB_ST_RELEASE_S32(chain_done, f + 1);   // L_f, M_f and the inverse pivots of block f are in shared memory
-                        }
-                        PH_MARK(6);
-                    } else {
-                        // ---- warps 1..7: eliminate the inverse depths on the fp64 tensor cores ---------------------------
-                        //   S = Hxx - W' W'^T,  rhs_x -= W' (w g_l),  W'[a][f] = W[a][f] / sqrt(h_f + mu D_f^2)
-                        // W' is staged through shared memory 32 features at a time as an 80-row tile whose row 78 carries
-                        // g_l / sqrt(h + mu D^2) (so that column 78 of the Gram matrix is the rhs update) and row 79 is zero.
-                        // The 55 upper 8x8 blocks of the 80x80 Gram matrix go to the 7 warps as row strips (SCPlan, compile-time).
-                        const int t2 = tid - 32, n2 = SOLVE_THREADS - 32;
-                        const int wq = (tid >> 5) - 1, lane = tid & 31;
-                        const int LDW = SC_LDW;
-                        double *tw = s.Ju;                         // 80 x 36 tile (aliases Ju .. red, unused during the solve)
-                        double *sinv = nF <= 1024 ? s.wj : lamc + F;   // 1 / sqrt(h + mu D^2): shared memory (wj: 1024 doubles) up to the reference's NUM_OF_F,
-                                                                       // the ninth workspace vector for the larger synthetic stress windows
-                        {   // Cauchy point: v_x^T Hxx v_x + 2 v_x^T Hxy v_y + lambda terms (H still unregularised / unfactored here)
-                            const double *v = s.stp;
-                            double pv = 0.0;
-                            for (int k = t2; k < NX * NX; k += n2) pv += v[k / NX] * s.Hxx[k] * v[k % NX];
-                            for (int k = t2; k < NX * NY; k += n2) pv += 2.0 * v[k / NY] * s.Hxy[k] * v[NX + k % NY];
-                            for (int f = t2; f < nF; f += n2) {
-                                double wv = 0.0;
-                                for (int a = 0; a < NX; a++) wv += W[(size_t)a * F + f] * v[a];
-                                pv += 2.0 * stl[f] * wv + hh[f] * stl[f] * stl[f];
-                            }
-                            for (int o = 16; o > 0; o >>= 1) pv += __shfl_sync(0xffffffffu, pv, (lane + o) & 31);
-                            if (lane == 0) s.lin[wq] = pv;
-                            CERB_BAR_SYNC(1, n2);
-                            for (int k = t2; k < NX; k += n2) s.Hxx[k * NX + k] += mu * s.D[k] * s.D[k];
-                        }
-                        PH_MARK_T(19, 32);
-                        for (int f = t2; f < nF; f += n2) sinv[f] = rsqrt(hh[f] + mu * Dl[f] * Dl[f]);
-                        double acc[8][2];
-                        _Pragma("unroll")
-                        for (int k = 0; k < 8; k++) { acc[k][0] = 0.0; acc[k][1] = 0.0; }
-                        CERB_BAR_SYNC(1, n2);
-                        // raw W / g_l values of a tile are fetched into registers one tile ahead (12 per thread: the loads are issued
-                        // together and stay in flight during the tensor-core loop), scaled and stored when the tile buffer is free
-                        double buf[12];
-                        auto fetch = [&](int f0) {
-                            const int nf = (nF - f0) < 32 ? (nF - f0) : 32;
-                            _Pragma("unroll")
-                            for (int u = 0; u < 12; u++) {
-                                const int e = t2 + u * n2, a = e >> 5, f = e & 31;
-                                buf[u] = (e < 80 * 32 && f < nf) ? (a < NX ? W[(size_t)a * F + f0 + f] : (a == NX ? gl[f0 + f] : 0.0)) : 0.0;
-                            }
-                        };
-                        fetch(0);
-                        PH_MARK_T(37, 32);
-                        for (int f0 = 0; f0 < nF; f0 += 32) {
-                            const int nf = (nF - f0) < 32 ? (nF - f0) : 32;
-                            _Pragma("unroll")
-                            for (int u = 0; u < 12; u++) {
-                                const int e = t2 + u * n2, a = e >> 5, f = e & 31;
-                                if (e < 80 * 32) tw[a * LDW + f] = (f < nf) ? buf[u] * sinv[f0 + f] : 0.0;
-                            }
-                            CERB_BAR_SYNC(1, n2);
-                            PH_MARK_T(38, 32);
-                            if (f0 + 32 < nF) fetch(f0 + 32);
-                            switch (wq) {                                  // warp-uniform; block plan per warp: SCPlan
-                                case 0: schur_tile<0>(tw, acc, lane); break;
-                                case 1: schur_tile<1>(tw, acc, lane); break;
-                                case 2: schur_tile<2>(tw, acc, lane); break;
-                                case 3: schur_tile<3>(tw, acc, lane); break;
-                                case 4: schur_tile<4>(tw, acc, lane); break;
-                                case 5: schur_tile<5>(tw, acc, lane); break;
-                                default: schur_tile<6>(tw, acc, lane); break;
-                            }
-                            CERB_BAR_SYNC(1, n2);
-                            PH_MARK_T(39, 32);
-                        }
-                        switch (wq) {
-                            case 0: schur_scatter<0>(s, acc, lane); break;
-                            case 1: schur_scatter<1>(s, acc, lane); break;
-                            case 2: schur_scatter<2>(s, acc, lane); break;
-                            case 3: schur_scatter<3>(s, acc, lane); break;
-                            case 4: schur_scatter<4>(s, acc, lane); break;
-                            case 5: schur_scatter<5>(s, acc, lane); break;
-                            default: schur_scatter<6>(s, acc, lane); break;
-                        }
-                        PH_MARK_T(7, 32);
-                        // ---- T = L^-1 Hyx (row a of Hxy in place; row 79: the y part of the rhs), rows on threads 32..111: block f
-                        // of the forward substitution starts as soon as warp 0 has published the factor of block f, so that the
-                        // substitution finishes right behind the chain instead of after it ----
-                        if (t2 <= NX) {
-                            double *row = (t2 < NX) ? s.Hxy + t2 * NY : s.yv + NX;
-                            double tp[NYB];
-                            _Pragma("unroll")
-                            for (int k = 0; k < NYB; k++) tp[k] = 0.0;
-                            _Pragma("unroll 1")
-                            for (int f = 0; f < NFR; f++) {
-                                while (CERB_LD_ACQUIRE_S32(chain_done) <= f) { CERB_SPIN_PAUSE(); }
-                                __threadfence_block();
-                                const double *L = s.Ad + f * 169, *idg = s.idg + NYB * f;
-                                double *t = row + NYB * f;
-                                double tc[NYB];
-                                _Pragma("unroll")
-                                for (int r = 0; r < NYB; r++) tc[r] = t[r];
-                                if (f > 0) {
-                                    const double *M = s.Bo + (f - 1) * 169;
-                                    _Pragma("unroll")
-                                    for (int r = 0; r < NYB; r++) { double acc = 0.0; _Pragma("unroll") for (int q = 0; q < NYB; q++) acc += M[r * NYB + q] * tp[q]; tc[r] -= acc; }
-                                }
-                                _Pragma("unroll")
-                                for (int c = 0; c < NYB; c++) {             // right-looking: the dependency chain is 13 (multiply, update) steps
-                                    tc[c] *= idg[c];
-                                    _Pragma("unroll")
-                                    for (int r = c + 1; r < NYB; r++) tc[r] -= L[r * NYB + c] * tc[c];
-                                }
-                                _Pragma("unroll")
-                                for (int r = 0; r < NYB; r++) { t[r] = tc[r]; tp[r] = tc[r]; }
-                            }
-                        }
-                    }
-                    __syncthreads();
-                    if (tid == 0) {
-                        double vhv = sca[S_VHV];
-                        for (int k = 0; k < 7; k++) vhv += s.lin[k];
-                        sca[S_ALPHA] = sca[S_GNORM2] / vhv;
-                    }
-                    PH_MARK(5);
-                    // (T = L^-1 Hyx was computed by warps 1..3 behind the chain factorisation, see above)
-                    __syncthreads();
-                    PH_MARK(8);
-                    // ---- S' = S - T T^T (lower), rhs'_x = rhs_x - T gy' : Gram matrix of the 79 x 143 matrix [T; gy'^T] on the
-                    // fp64 tensor cores, K = 143 padded to 144; block rectangles per warp, see ttt_warp ----------
-                    switch (tid >> 5) {
-                        case 0: ttt_warp<0>(s, tid & 31); break;
-                        case 1: ttt_warp<1>(s, tid & 31); break;
-                        case 2: ttt_warp<2>(s, tid & 31); break;
-                        case 3: ttt_warp<3>(s, tid & 31); break;
-                        case 4: ttt_warp<4>(s, tid & 31); break;
-                        case 5: ttt_warp<5>(s, tid & 31); break;
-                        case 6: ttt_warp<6>(s, tid & 31); break;
-                        default: ttt_warp<7>(s, tid & 31); break;
-                    }
-                    __syncthreads();
-                    PH_MARK(9);
-                    // ---- dense Cholesky of the 79 x 79 lower triangle, rhs carried as row 79 (z = L^-1 rhs), blocked by panels of 8,
-                    // with look-ahead: (a) warp 0 factors a diagonal block in registers (pivots / column entries exchanged by shuffles),
-                    // (b) one thread per row below solves its 8 panel entries against L_kk, (c) the trailing lower triangle is updated
-                    // block by block on the fp64 tensor cores (A_ij -= L_ik L_jk^T, K = 8) -- warp 0 takes only the block that becomes
-                    // the next diagonal block and factors it right away, while warps 1..7 update the rest.  Two barriers per panel; the
-                    // serial column sweeps of the diagonal blocks (the critical path) overlap with the trailing updates.
-                    {
-                        const int wq = tid >> 5, lane = tid & 31;
-                        auto factor_diag = [&](int c0, int nb, double *Lkk) {      // warp 0: L_kk of the nb x nb block at (c0, c0); Lkk[64..72) = 1 / diag
-                            const bool act = lane < nb;
-                            const int r = act ? lane : 0;
-                            double a[8];
-                            _Pragma("unroll")
-                            for (int c = 0; c < 8; c++) a[c] = (c < nb && c <= r) ? s.Hxx[(c0 + r) * NX + c0 + c] : 0.0;
-                            double myinv = 1.0;
-                            _Pragma("unroll")
-                            for (int j = 0; j < 8; j++) {
-                                double d = __shfl_sync(0xffffffffu, a[j], j);
-                                if (j < nb && !(d > 0.0)) { if (lane == 0) sca[S_OK] = 0; }
-                                if (!(d > 0.0)) d = 1.0;
-                                const double inv = rsqrt(d);
-                                if (lane == j) myinv = inv;
-                                const double l = (lane == j) ? d * inv : a[j] * inv;
-                                a[j] = l;
-                                _Pragma("unroll")
-                                for (int k = j + 1; k < 8; k++) { const double lk = __shfl_sync(0xffffffffu, l, k); a[k] -= l * lk; }
-                            }
-                            if (act) {
-                                _Pragma("unroll")
-                                for (int c = 0; c < 8; c++) if (c <= r) { s.Hxx[(c0 + r) * NX + c0 + c] = a[c]; Lkk[r * 8 + c] = a[c]; }
-                                Lkk[64 + r] = myinv; s.idx[c0 + r] = myinv;
-                            }
-                        };
-                        auto trailing_block = [&](int c0, int b0, int b) {          // block b = (bi, bj), bj <= bi, of the rows / columns from 8 b0 on
-                            int bi = 0, idx = b;
-                            while (idx > bi) { idx -= bi + 1; bi++; }
-                            const int ri = 8 * (b0 + bi) + (lane >> 2), rj = 8 * (b0 + idx) + (lane >> 2);
-                            double a0 = 0.0, a1 = 0.0;
-                            for (int ks = 0; ks < 2; ks++) {
-                                const int cc = c0 + 4 * ks + (lane & 3);
-                                const double av = (ri < NX) ? s.Hxx[ri * NX + cc] : (ri == NX ? s.yv[cc] : 0.0);
-                                const double bv = (rj < NX) ? s.Hxx[rj * NX + cc] : 0.0;
-                                CERB_DMMA(a0, a1, av, bv, a0, a1);
-                            }
-                            const int cj = 8 * (b0 + idx) + 2 * (lane & 3);
-                            if (ri < NX) {
-                                if (cj <= ri && cj < NX) s.Hxx[ri * NX + cj] -= a0;
-                                if (cj + 1 <= ri && cj + 1 < NX) s.Hxx[ri * NX + cj + 1] -= a1;
-                            } else if (ri == NX) {
-                                if (cj < NX) s.yv[cj] -= a0;
-                                if (cj + 1 < NX) s.yv[cj + 1] -= a1;
-                            }
-                        };
-                        if (wq == 0) factor_diag(0, 8, s.red);
+                for (;;) {
+                    if (!(sca[S_MU] < 1.0)) {                 // while (mu_ < max_mu_) not entered: LINEAR_SOLVER_FAILURE without a solve
                         __syncthreads();
-                        int pk = 0;
-                        for (int c0 = 0; c0 < NX; c0 += 8, pk ^= 1) {
-                            const int nb = (NX - c0) < 8 ? (NX - c0) : 8, c1 = c0 + nb;
-                            const double *Lkk = s.red + 80 * pk;            // factored diagonal block of this panel (+ inverse diagonal at [64..72))
-                            // (b) rows c1 .. NX (row NX = rhs, kept in yv)
-                            if (tid <= NX - c1) {
-                                const int i = c1 + tid;
-                                double *row = (i < NX) ? s.Hxx + i * NX + c0 : s.yv + c0;
-                                double t[8];
-                                _Pragma("unroll")
-                                for (int c = 0; c < 8; c++) t[c] = (c < nb) ? row[c] : 0.0;
-                                _Pragma("unroll")
-                                for (int c = 0; c < 8; c++) {
-                                    if (c < nb) {
-                                        t[c] *= Lkk[64 + c];
-                                        _Pragma("unroll")
-                                        for (int c2 = c + 1; c2 < 8; c2++) if (c2 < nb) t[c2] -= t[c] * Lkk[c2 * 8 + c];
-                                    }
-                                }
-                                _Pragma("unroll")
-                                for (int c = 0; c < 8; c++) if (c < nb) row[c] = t[c];
-                            }
-                            __syncthreads();
-                            if (c1 >= NX) break;
-                            // (c) trailing update of rows / columns c1 .. NX (row NX = rhs) + look-ahead factorisation of the next diagonal block
-                            {
-                                const int b0 = c1 >> 3, nbt = 10 - b0;               // block rows b0 .. 9
-                                const int nblk = nbt * (nbt + 1) / 2;
-                                if (wq == 0) {
-                                    trailing_block(c0, b0, 0);
-                                    __syncwarp();
-                                    factor_diag(c1, (NX - c1) < 8 ? (NX - c1) : 8, s.red + 80 * (pk ^ 1));
-                                } else {
-                                    for (int b = wq; b < nblk; b += 7) trailing_block(c0, b0, b);
-                                }
-                            }
-                            __syncthreads();
-                        }
+                        if (tid == 0) { sca[S_OK] = 0; sca[S_REUSE] = 1; }
+                        __syncthreads();
+                        break;
                     }
-                    PH_MARK(10);
-                    // ---- back substitution L^T y_x = z by warp 0: lane holds y[lane], y[lane + 32], y[lane + 64] in registers;
-                    // branch-free steps (selects), the L entries of the next step are loaded before the current shuffle completes ----
-                    if (tid < 32) {
-                        double y0 = s.yv[tid], y1 = s.yv[32 + tid], y2 = (64 + tid < NX) ? s.yv[64 + tid] : 0.0;
-                        _Pragma("unroll 1")
-                        for (int k = NX - 1; k >= 0; k--) {
-                            const double *Lk = s.Hxx + k * NX;
-                            const double ik = s.idx[k];
-                            const double l0 = (tid < k) ? Lk[tid] : 0.0, l1 = (32 + tid < k) ? Lk[32 + tid] : 0.0, l2 = (64 + tid < k) ? Lk[64 + tid] : 0.0;
-                            const double src = (k >= 64) ? y2 : (k >= 32 ? y1 : y0);
-                            const double yk = __shfl_sync(0xffffffffu, src, k & 31) * ik;
-                            y0 = (tid == k) ? yk : y0 - l0 * yk;
-                            y1 = (32 + tid == k) ? yk : y1 - l1 * yk;
-                            y2 = (64 + tid == k) ? yk : y2 - l2 * yk;
-                        }
-                        s.yv[tid] = y0; s.yv[32 + tid] = y1; if (64 + tid < NX) s.yv[64 + tid] = y2;
-                    }
+                    dogleg_diagonal(s, c, tid PH_FWD);
+                    gauss_newton_step(P, s, c, pc, gn_attempts, tid PH_FWD);
+                    if (tid == 0) sca[S_REUSE] = 1;
                     __syncthreads();
-                    if (has_prior) {                                                                         // the factor of Hxx is dead from here on
-                        if (bulk_ok) { if (tid == 0) CERB_BULK_G2S(s.Hxx, pimg, PIMG_HXY * 8, &s.mbar[0]); }
-                        else copy_g2s_async(s.Hxx, pimg, HXX_SZ, tid);
-                        hxx_prefetched = true;
-                    }
-                    PH_MARK(11);
-                    // ---- y part: u = gy' - T^T y_x, then L^T y_y = u blockwise (warp 0) ------------------------------------
-                    for (int q = tid; q < NY; q += SOLVE_THREADS) { double t = 0.0; for (int a = 0; a < NX; a++) t += s.Hxy[a * NY + q] * s.yv[a]; s.yv[NX + q] -= t; }
+                    if (sca[S_OK] != 0.0) break;              // the Gauss-Newton step is there
                     __syncthreads();
-                    if (tid < 32) {      // lane r holds component r of the current block; one shuffle per substitution step
-                        const int r = tid < NYB ? tid : 0;
-                        double yn[NYB];                                  // solved block f + 1 (all lanes)
-                        _Pragma("unroll")
-                        for (int k = 0; k < NYB; k++) yn[k] = 0.0;
-                        _Pragma("unroll 1")
-                        for (int f = NFR - 1; f >= 0; f--) {
-                            const double *L = s.Ad + f * 169;
-                            double u = s.yv[NX + NYB * f + r];
-                            if (f < NFR - 1) {
-                                const double *M = s.Bo + f * 169;
-                                double t = 0.0;
-                                _Pragma("unroll")
-                                for (int k = 0; k < NYB; k++) t += M[k * NYB + r] * yn[k];
-                                u -= t;
-                            }
-                            double lc[NYB], ig[NYB];                          // column r of L^T and the inverse pivots: loaded before the chain
-                            _Pragma("unroll")
-                            for (int k = 0; k < NYB; k++) { lc[k] = (tid < k) ? L[k * NYB + r] : 0.0; ig[k] = s.idg[NYB * f + k]; }
-                            _Pragma("unroll")
-                            for (int k = NYB - 1; k >= 0; k--) {
-                                const double yk = __shfl_sync(0xffffffffu, u, k) * ig[k];
-                                yn[k] = yk;
-                                u = (tid == k) ? yk : u - lc[k] * yk;
-                            }
-                            if (tid < NYB) s.yv[NX + NYB * f + tid] = u;
-                        }
-                    }
+                    if (tid == 0) sca[S_MU] *= 10.0;           // mu_ *= mu_increase_factor_; continue;
                     __syncthreads();
-                    PH_MARK(12);
-                    // ---- inverse depths: y_l = (gl - w^T y_x) / (h + mu D^2) ; validity ---------------------------------------
-                    double bad = 0.0;
-                    for (int f = tid; f < nF; f += SOLVE_THREADS) {
-                        double t = gl[f];
-                        for (int a = 0; a < NX; a++) t -= W[(size_t)a * F + f] * s.yv[a];
-                        const double y = t / (hh[f] + mu * Dl[f] * Dl[f]);
-                        gnl[f] = y;
-                        if (!(fabs(y) < 1e300)) bad = 1.0;
-                    }
-                    for (int k = tid; k < NR; k += SOLVE_THREADS) if (!(fabs(s.yv[k]) < 1e300)) bad = 1.0;
-                    if (bad != 0.0) sca[S_OK] = 0;          // benign race: every writer stores 0
-                    if (gn_attempts < P.test_fail_factorizations) sca[S_OK] = 0;      // fault injection of the parity tests (0 in production)
-                    gn_attempts++;
-                    __syncthreads();
-                    PH_MARK(13);
+                    if (!(sca[S_MU] < 1.0)) break;            // LINEAR_SOLVER_FAILURE (S_OK == 0)
+                    linearize(P, s, c, pc, s.xs, c.lam, false, tid PH_FWD);      // the failed in-place factorisation overwrote H: rebuild it
                 }
-                if (sca[S_OK] != 0.0) {
-                    // gauss_newton_step = -D * y ; norms for the dogleg
-                    double part3[2] = {0.0, 0.0};    // ||gn||^2, gh . gn
-                    for (int k = tid; k < NR; k += SOLVE_THREADS) { const double v = -s.D[k] * s.yv[k]; s.gn[k] = v; part3[0] += v * v; part3[1] += s.gh[k] * v; }
-                    for (int f = tid; f < nF; f += SOLVE_THREADS) { const double v = -Dl[f] * gnl[f]; gnl[f] = v; part3[0] += v * v; part3[1] += ghl[f] * v; }
-                    double tot3[2];
-                    block_sum<2>(part3, s.red, tot3, tid);
-                    if (tid == 0) { sca[S_GNNORM2] = tot3[0]; sca[S_GDOTGN] = tot3[1]; }
-                    __syncthreads();
-                }
-                if (tid == 0) sca[S_REUSE] = 1;
-                __syncthreads();
-                if (sca[S_OK] != 0.0) break;              // the Gauss-Newton step is there
-                __syncthreads();
-                if (tid == 0) sca[S_MU] *= 10.0;           // mu_ *= mu_increase_factor_; continue;
-                __syncthreads();
-                if (!(sca[S_MU] < 1.0)) break;            // LINEAR_SOLVER_FAILURE (S_OK == 0)
-                linearize(s.xs, lam, false);               // the failed in-place factorisation overwrote H: rebuild it at the same point
-              }
             }
-            // =============================== step validity =================================================
-            if (sca[S_OK] == 0.0) {       // LINEAR_SOLVER_FAILURE -> HandleInvalidStep
-                if (tid == 0) {
-                    sca[S_INVALID] += 1;
-                    if (sca[S_INVALID] >= 5) { sca[S_DONE] = 1; sca[S_TERM] = 2; }
-                    sca[S_MU] *= 10.0; sca[S_REUSE] = 0;      // StepIsInvalid
-                }
-                __syncthreads();
-                if (sca[S_DONE] != 0.0) break;
-                need_linearize = true;     // the failed factorisation overwrote H; rebuild it at the same point
-                continue;
-            }
-            // =============================== ComputeTraditionalDoglegStep ====================================
-            if (tid == 0) {
-                const double radius = sca[S_RADIUS], alpha = sca[S_ALPHA];
-                const double gradient_norm = sqrt(sca[S_GNORM2]), gauss_newton_norm = sqrt(sca[S_GNNORM2]);
-                double p, q, nrm;
-                if (gauss_newton_norm <= radius) { p = 0.0; q = 1.0; nrm = gauss_newton_norm; }
-                else if (gradient_norm * alpha >= radius) { p = -(radius / gradient_norm); q = 0.0; nrm = radius; }
-                else {
-                    const double b_dot_a = -alpha * sca[S_GDOTGN];
-                    const double a_squared_norm = (alpha * gradient_norm) * (alpha * gradient_norm);
-                    const double b_minus_a_squared_norm = a_squared_norm - 2 * b_dot_a + gauss_newton_norm * gauss_newton_norm;
-                    const double c = b_dot_a - a_squared_norm;
-                    const double d = sqrt(c * c + b_minus_a_squared_norm * (radius * radius - a_squared_norm));
-                    const double beta = (c <= 0) ? (d - c) / b_minus_a_squared_norm : (radius * radius - a_squared_norm) / (d + c);
-                    p = -alpha * (1.0 - beta); q = beta;
-                    nrm = sqrt(p * p * sca[S_GNORM2] + 2 * p * q * sca[S_GDOTGN] + q * q * sca[S_GNNORM2]);
-                }
-                sca[S_P] = p; sca[S_Q] = q; sca[S_DLNORM] = nrm;
-                // model_cost_change = -(step^T g~ + 0.5 step^T H~ step) with step = (p gh + q gn) / D, using
-                // H~ (gn/D) = -(g~ + mu D gn)  (the Gauss-Newton equations):
-                const double mu = sca[S_MU], g2 = sca[S_GNORM2], gg = sca[S_GDOTGN], n2 = sca[S_GNNORM2];
-                const double sTg = p * g2 + q * gg;
-                const double sHs = p * p * (g2 / alpha) - 2.0 * p * q * (g2 + mu * gg) + q * q * (-gg - mu * n2);
-                sca[S_MODEL] = -(sTg + 0.5 * sHs);
-            }
-            __syncthreads();
-            if (!(sca[S_MODEL] > 0.0)) {   // invalid step
-                if (tid == 0) {
-                    sca[S_INVALID] += 1;
-                    if (sca[S_INVALID] >= 5) { sca[S_DONE] = 1; sca[S_TERM] = 2; }
-                    sca[S_MU] *= 10.0; sca[S_REUSE] = 0;
-                }
-                __syncthreads();
-                if (sca[S_DONE] != 0.0) break;
-                need_linearize = true;     // the factorisation overwrote H; rebuild it at the same point
-                continue;
-            }
+            if (sca[S_OK] == 0.0) { if (handle_invalid_step(sca, tid)) break; need_linearize = true; continue; }      // LINEAR_SOLVER_FAILURE
+            dogleg_step(sca, tid);
+            if (!(sca[S_MODEL] > 0.0)) { if (handle_invalid_step(sca, tid)) break; need_linearize = true; continue; }
             if (tid == 0) sca[S_INVALID] = 0;
-            // delta = ((p gh + q gn) / D) * jacobi_scale
-            {
-                const double p = sca[S_P], q = sca[S_Q];
-                for (int k = tid; k < NR; k += SOLVE_THREADS) s.stp[k] = (p * s.gh[k] + q * s.gn[k]) / s.D[k] * s.sc[k];
-                for (int f = tid; f < nF; f += SOLVE_THREADS) stl[f] = (p * ghl[f] + q * gnl[f]) / Dl[f] * sl[f];
-            }
-            __syncthreads();
-            // =============================== candidate point and its cost ===================================
-            PH_MARK(14);
-            apply_plus(s, s.stp, lam, stl, lamc, nF, ex_open, td_open, tid);
-            // Speculative linearisation: if the previous step of this window was accepted, the candidate is linearised right away --
-            // its cost is the candidate cost, and when the step is accepted (the common case) the linearisation of the next iteration
-            // is already there, so the separate cost-only pass is saved.  A rejected step leaves H / g / W at the candidate, which is
-            // harmless: the re-use path of the dogleg needs none of them.  Not done for the last allowed iteration (never needed).
             const bool speculate = last_accepted && iteration < P.max_iters;
-            {
-                double part[2];
-                PH_MARK(15);
-                if (speculate) { linearize(s.xc, lamc, false); part[0] = 0.0; }
-                else {
-                    load_geometry(s.xc, s, tid);
-                    part[0] = vision_cost(P, w, s.xc, lamc, tid);
-                    PH_MARK(16);
-                    part[0] += inertial_cost(P, w, s.xc, tid);
-                }
-                PH_MARK(17);
-                part[1] = ambient_sq(s.xs, s.xc, lam, lamc, nF, ex_open, lb_open, td_open, tid);
-                double tot[2];
-                block_sum<2>(part, s.red, tot, tid);
-                if (tid == 0) {
-                    double cc = speculate ? sca[S_LCOST] : tot[0];
-                    if (!(cc == cc) || fabs(cc) > 1e300) cc = 1.7976931348623157e308;
-                    sca[S_CCOST] = cc; sca[S_STEPNORM] = sqrt(tot[1]);
-                }
-            }
+            evaluate_candidate(P, s, c, pc, speculate, tid PH_FWD);
+            if (accept_or_reject(P, sca, tid)) break;
+            const bool accepted = (sca[S_OK] == 2.0);
             __syncthreads();
-            // =============================== tolerances, accept / reject =====================================
-            bool accepted = false;
-            if (tid == 0) {
-                const double x_cost = sca[S_XCOST], cand = sca[S_CCOST];
-                if (sca[S_STEPNORM] <= P.ptol * (sca[S_XNORM] + P.ptol)) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
-                else if (fabs(x_cost - cand) <= P.ftol * x_cost) { sca[S_DONE] = 1; sca[S_TERM] = 0; }
-                else {
-                    const double rel = (x_cost - cand) / sca[S_MODEL];
-                    if (rel > P.min_rel_dec) {            // StepAccepted
-                        if (rel < 0.25) sca[S_RADIUS] *= 0.5;
-                        if (rel > 0.75) sca[S_RADIUS] = fmax(sca[S_RADIUS], 3.0 * sca[S_DLNORM]);
-                        sca[S_MU] = fmax(1e-8, 2.0 * sca[S_MU] / 10.0);
-                        sca[S_REUSE] = 0; sca[S_NSUCC] += 1; sca[S_OK] = 2;     // 2 == accepted marker
-                        sca[S_XCOST] = cand;                                   // x_cost of the new point (re-evaluated by the next linearisation, if any)
-                    } else {                              // StepRejected
-                        sca[S_RADIUS] *= 0.5; sca[S_REUSE] = 1; sca[S_OK] = 1;
-                    }
-                }
-            }
-            __syncthreads();
-            if (sca[S_DONE] != 0.0) break;
-            accepted = (sca[S_OK] == 2.0);
-            __syncthreads();
-            if (accepted) {
+            if (accepted) {      // the candidate becomes the current point
                 for (int k = tid; k < ST_STRIDE; k += SOLVE_THREADS) s.xs[k] = s.xc[k];
-                for (int f = tid; f < nF; f += SOLVE_THREADS) lam[f] = lamc[f];
+                for (int f = tid; f < c.nF; f += SOLVE_THREADS) c.lam[f] = ws.lamc[f];
                 if (tid == 0) { sca[S_OK] = 1; if (speculate) { sca[S_XNORM] = sca[S_LNORM]; sca[S_GMAX] = sca[S_LGMAX]; } }
                 __syncthreads();
                 need_linearize = !speculate;                     // a speculative linearisation is the linearisation at the new point
@@ -1659,7 +1689,7 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, CERB_SOLVE_MIN_BLOCKS) vilo_so
             PH_MARK(18);
         }
         // ---- write back ---------------------------------------------------------------------------------
-        if (bulk_ok && hxx_prefetched) { CERB_MBAR_WAIT(&s.mbar[0], par0); par0 ^= 1; }   // drain a prefetch of the prior image that was never consumed
+        if (c.bulk_ok && pc.hxx_prefetched) { CERB_MBAR_WAIT(&s.mbar[0], pc.par0); pc.par0 ^= 1; }   // drain a prefetch of the prior image that was never consumed
         CERB_CP_ASYNC_WAIT();
         for (int k = tid; k < ST_SIZE; k += SOLVE_THREADS) P.state[(size_t)w * ST_STRIDE + k] = s.xs[k];
         if (tid == 0) {
@@ -1670,7 +1700,6 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, CERB_SOLVE_MIN_BLOCKS) vilo_so
         __syncthreads();
     }
 }
-
 
 // ---- marginalization: A = sum J^T J, b = sum J^T r over the factors that touch the dropped blocks ----------------------------------
 // MarginalizationInfo::{addResidualBlockInfo, preMarginalize, marginalize} up to ThreadsConstructA (marginalization_factor.cpp:98-279)
@@ -1697,36 +1726,12 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, 1) marg_assemble_kernel(CERB_G
     CERB_DYN_SMEM(double, smem_base);
     Smem s; smem_carve(smem_base, s);
     const int tid = threadIdx.x, F = P.maxF;
-    double *ws = P.ws + (size_t)blockIdx.x * P.ws_stride;
-    double *W = ws + ws_W(F);
-    double *hh = ws + ws_vecs(F), *gl = hh + F, *sl = gl + F;
-    int *chunks = reinterpret_cast<int *>(ws + ws_chunks(F));
-    double *pimg = ws + ws_prior(F);
+    const CtaWs ws = ws_carve(P);
     int *colx = reinterpret_cast<int *>(s.idx);           // [79] column of x index a in A (-1: block absent), then [26] of the y indices of frames 0 / 1
                                                           // (idx: 80 doubles that only the Gauss-Newton step of the solver uses; idg holds the dummy slots of the IMU scatter)
     int *coly = colx + 80;
     int *misc = coly + 32;                                // [0] n0, [1] m, [2] n, [3] status, [4] stereo seen, [5] longest anchor-0 track
-    if (tid < 32) {                                       // scatter plan of the IMU-leg Gram matrix (same as in vilo_solve_kernel)
-        int *plan = reinterpret_cast<int *>(ws + ws_imuplan(F));
-        int q = 0;
-        for (int mi = 0; mi < 5; mi++)
-            for (int ni = mi; ni < 5; ni++, q++)
-                for (int e = 0; e < 2; e++) {
-                    const int la = 8 * mi + (tid >> 2), lb = 8 * ni + 2 * (tid & 3) + e;
-                    int px = (int)(s.idg - smem_base) + tid, py = 256 << 12;
-                    if (la <= lb && lb <= 38 && la != 38) {
-                        double *p0[2], *p1[2];
-                        for (int i = 0; i < 2; i++) {
-                            const int da = imu_col_dest(i, la);
-                            if (lb == 38) { p0[i] = da >= 0 ? s.g + da : s.g + NX + (-da - 1); p1[i] = nullptr; }
-                            else scatter_addr(s, da, imu_col_dest(i, lb), &p0[i], &p1[i]);
-                        }
-                        px = (int)(p0[0] - smem_base);
-                        py = (int)(p0[1] - p0[0]) | (((p1[0] ? (int)(p1[0] - p0[0]) : 0) + 256) << 12);
-                    }
-                    plan[(2 * (q * 2 + e)) * 32 + tid] = px; plan[(2 * (q * 2 + e) + 1) * 32 + tid] = py;
-                }
-    }
+    build_imu_plan(s, smem_base, ws.imu_plan, tid);
     __syncthreads();
     for (int w = blockIdx.x; w < P.n_windows; w += gridDim.x) {
         const int nF = P.n_features[w], flag = M.flags[w];
@@ -1738,18 +1743,11 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, 1) marg_assemble_kernel(CERB_G
         if (tid == 0) {
             int n0 = 0;
             if (flag == MARG_OLD) while (n0 < nF && fstart[n0] == 0) n0++;
-            int n = 0, c0 = 0;
-            while (c0 < n0) {
-                const int e = (c0 + 64 < n0) ? c0 + 64 : n0;
-                chunks[1 + n] = c0;
-                if (n < 15) { s.ti[97 + 2 * n] = c0; s.ti[98 + 2 * n] = ((e - c0) << 8) | 0; }
-                n++; c0 = e;
-            }
-            chunks[1 + n] = n0; chunks[0] = n; s.ti[96] = n;
-            s.ti[131] = flag == MARG_OLD ? 1 : 2;
+            build_chunks(fstart, s, ws.chunks, n0);                  // all anchored at frame 0: chunks of 64
+            s.ti[TI_IMU_MASK] = flag == MARG_OLD ? 1 : 2;
             misc[0] = n0; misc[4] = 0; misc[5] = 0;
         }
-        const bool has_prior = build_prior_image(P, s, w, pimg, tid);
+        const bool has_prior = build_prior_image(P, s, w, ws.pimg, tid);
         for (int k = tid; k < ST_STRIDE; k += SOLVE_THREADS) s.xs[k] = (k < ST_SIZE) ? M.state[(size_t)w * ST_STRIDE + k] : 0.0;
         __syncthreads();
         const int n0 = misc[0];
@@ -1763,13 +1761,13 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, 1) marg_assemble_kernel(CERB_G
         }
         // ---- linearise: prior image | visual factors of the anchor-0 tracks | IMU-leg factor 0 | prior gradient ---------------------
         if (!has_prior) { for (int k = tid; k < HXX_SZ; k += SOLVE_THREADS) s.Hxx[k] = 0.0; }
-        else copy_g2s(s.Hxx, pimg, HXX_SZ, tid);
+        else copy_g2s(s.Hxx, ws.pimg, HXX_SZ, tid);
         for (int k = tid; k < NRP; k += SOLVE_THREADS) s.g[k] = 0.0;
         load_geometry(s.xs, s, tid);
-        if (n0 > 0) vision_linearize(P, w, s.xs, lam, W, hh, gl, sl, false, chunks, tid);
+        if (n0 > 0) vision_linearize(P, w, s.xs, lam, ws.W, ws.hh, ws.gl, ws.sl, false, ws.chunks, tid);
         __syncthreads();
-        if (has_prior) copy_g2s(s.Hxy, pimg + PIMG_HXY, PIMG_REST, tid);
-        else for (int k = tid; k < HXY_SZ + 1859 + 1690; k += SOLVE_THREADS) s.Hxy[k] = 0.0;
+        if (has_prior) copy_g2s(s.Hxy, ws.pimg + PIMG_HXY, PIMG_REST, tid);
+        else for (int k = tid; k < PIMG_REST; k += SOLVE_THREADS) s.Hxy[k] = 0.0;
         __syncthreads();
         inertial_linearize(P, w, s.xs, tid);
         // ---- block presence and the [dropped | kept] column map ---------------------------------------------------------------
@@ -1839,14 +1837,14 @@ CERB_GLOBAL void __launch_bounds__(SOLVE_THREADS, 1) marg_assemble_kernel(CERB_G
             for (int e = tid; e < 26 * 26; e += SOLVE_THREADS) {             // y - y
                 const int q = e / 26, r = e % 26, cq = coly[q], cr = coly[r]; if (cq < 0 || cr < 0) continue;
                 const int fq = q / NYB, fr = r / NYB, kq = q % NYB, kr = r % NYB;
-                A[(size_t)cq * pos + cr] = fq == fr ? s.Ad[fq * 169 + kq * NYB + kr] : (fq < fr ? s.Bo[kq * NYB + kr] : s.Bo[kr * NYB + kq]);
+                A[(size_t)cq * pos + cr] = fq == fr ? s.Ad[fq * HBLK + kq * NYB + kr] : (fq < fr ? s.Bo[kq * NYB + kr] : s.Bo[kr * NYB + kq]);
             }
             for (int e = tid; e < NX * n0; e += SOLVE_THREADS) {             // x - lambda
                 const int a = e / n0, k = e % n0, ca = colx[a]; if (ca < 0) continue;
-                const double v = W[(size_t)a * F + k];
+                const double v = ws.W[(size_t)a * F + k];
                 A[(size_t)ca * pos + l0 + k] = v; A[(size_t)(l0 + k) * pos + ca] = v;
             }
-            for (int k = tid; k < n0; k += SOLVE_THREADS) { A[(size_t)(l0 + k) * pos + l0 + k] = hh[k]; b[l0 + k] = gl[k]; }
+            for (int k = tid; k < n0; k += SOLVE_THREADS) { A[(size_t)(l0 + k) * pos + l0 + k] = ws.hh[k]; b[l0 + k] = ws.gl[k]; }
             for (int a = tid; a < NX; a += SOLVE_THREADS) if (colx[a] >= 0) b[colx[a]] = s.g[a];
             for (int q = tid; q < 26; q += SOLVE_THREADS) if (coly[q] >= 0) b[coly[q]] = s.g[NX + q];
         }
