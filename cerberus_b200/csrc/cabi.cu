@@ -30,8 +30,15 @@ static int fail(int code, const std::string &msg) { g_err = msg; return code; }
         if (e_ != cudaSuccess) return fail(CERB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_)); \
     } while (0)
 
-template <typename T> static cudaError_t dmalloc(T **p, size_t n) { return cudaMalloc((void **)p, n * sizeof(T)); }
-template <typename T> static cudaError_t hmalloc(T **p, size_t n) { return cudaMallocHost((void **)p, n * sizeof(T)); }
+// One array of the resident batch: `per` elements per window, window w at at(w); `h` is its pinned host mirror of the same shape, where it has one
+// (the staging of a caller's descriptors, the landing place of the results).
+template <typename T> struct Resident {
+    T *d = nullptr, *h = nullptr;
+    size_t per = 0;
+    T *at(size_t w) const { return d + w * per; }
+    T *h_at(size_t w) const { return h + w * per; }
+    size_t bytes(size_t n_windows) const { return n_windows * per * sizeof(T); }
+};
 
 struct CerbHandle {
     CerbSolverConfig cfg;
@@ -46,19 +53,18 @@ struct CerbHandle {
     double last_ms = 0; int last_launches = 0, last_dma_ops = 0; size_t last_staged_bytes = 0;
     int B = 0, F = 0, O = 0;          // capacities
     int n = 0;                        // windows currently resident
-    // device: the caller's descriptors as they are (filled by DMA) ...
-    CerbWindowDesc *d_rdesc = nullptr; CerbFeature *d_rfeat = nullptr; CerbObservation *d_robs = nullptr; CerbWindowState *d_rstate = nullptr;
-    double *d_rpre = nullptr, *d_rlam = nullptr;
-    // ... and the solver's layout (written by pack_kernel)
-    int *d_nfeat = nullptr, *d_fstart = nullptr, *d_fnobs = nullptr, *d_foff = nullptr, *d_flags = nullptr, *d_stereo = nullptr, *d_pmeta = nullptr, *d_repi = nullptr, *d_perm = nullptr;
-    double *d_obs = nullptr, *d_pre = nullptr, *d_sinfo = nullptr, *d_pJ = nullptr, *d_pr = nullptr, *d_px0 = nullptr, *d_pHp = nullptr;
-    double *d_state = nullptr, *d_state0 = nullptr, *d_lam = nullptr, *d_lam0 = nullptr, *d_repd = nullptr, *d_ws = nullptr, *d_dbg = nullptr, *d_G = nullptr, *d_probe_repd = nullptr;
+    // The resident batch, sized and allocated by create_impl.  The caller's descriptors as they are (filled by DMA, through the pinned mirror
+    // for sources that are not in registered memory) ...
+    Resident<CerbWindowDesc> rdesc; Resident<CerbFeature> rfeat; Resident<CerbObservation> robs; Resident<CerbWindowState> rstate;
+    Resident<double> rpre, rlam;
+    // ... the solver's layout (written by pack_kernel; the prior matrix and residuals by DMA) and its results ...
+    Resident<int> n_features, feat_start, feat_nobs, feat_off, flags, obs_stereo, prior_meta, rep_i, perm;
+    Resident<double> obs, pre, sinfo, prior_J, prior_r, prior_x0, prior_Hp, state, state0, lam, lam0, rep_d;
+    // ... and the results in the caller's layout (unpack_kernel), with pinned mirrors
+    Resident<double> olam, ostate; Resident<CerbSolveReport> orep;
+    double *d_ws = nullptr, *d_dbg = nullptr, *h_dbg = nullptr, *d_G = nullptr, *d_probe_repd = nullptr;
     int *d_probe_repi = nullptr;
-    double *d_olam = nullptr, *d_ostate = nullptr; CerbSolveReport *d_orep = nullptr;      // results in the caller's layout (unpack_kernel)
-    // pinned staging (used for sources that are not in registered memory, and for the results)
-    CerbWindowDesc *h_rdesc = nullptr; CerbFeature *h_rfeat = nullptr; CerbObservation *h_robs = nullptr; CerbWindowState *h_rstate = nullptr;
-    double *h_rpre = nullptr, *h_rlam = nullptr, *h_pJ = nullptr, *h_pr = nullptr, *h_state = nullptr, *h_lam = nullptr, *h_dbg = nullptr;
-    CerbSolveReport *h_orep = nullptr;
+    std::vector<void *> dev_bufs, host_bufs;    // everything create_impl allocated (cudaMalloc / cudaMallocHost): freed by cerb_destroy
     std::vector<std::pair<uintptr_t, size_t>> regs;   // host ranges registered with cerb_register_host_buffer: DMA straight out of them
     std::vector<int> nfeat, n0;       // [B] n_features / number of tracks anchored at frame 0 of the resident windows
     int test_fail_factorizations = 0; double test_initial_mu = 0.0;   // fault injection of the parity tests (environment, read by cerb_create)
@@ -128,6 +134,23 @@ int cerb_create(const CerbSolverConfig *cfg, CerbHandle **out) {
 
 }  // extern "C"
 
+template <typename T> static cudaError_t dmalloc(CerbHandle *h, T **p, size_t n) {
+    const cudaError_t e = cudaMalloc((void **)p, n * sizeof(T));
+    if (e == cudaSuccess) h->dev_bufs.push_back(*p);
+    return e;
+}
+template <typename T> static cudaError_t hmalloc(CerbHandle *h, T **p, size_t n) {
+    const cudaError_t e = cudaMallocHost((void **)p, n * sizeof(T));
+    if (e == cudaSuccess) h->host_bufs.push_back(*p);
+    return e;
+}
+// B windows of `per` elements, and the pinned mirror if `mirror`
+template <typename T> static cudaError_t alloc(CerbHandle *h, Resident<T> &a, size_t per, bool mirror = false) {
+    a.per = per;
+    const cudaError_t e = dmalloc(h, &a.d, (size_t)h->B * per);
+    return (e != cudaSuccess || !mirror) ? e : hmalloc(h, &a.h, (size_t)h->B * per);
+}
+
 static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDeviceProp &prop) {
     h->cfg = *cfg; h->sm_count = prop.multiProcessorCount;
     // Test hooks of the Ceres LINEAR_SOLVER_FAILURE path (tests/test_solver_failure.py); unset in production.  A factorisation of
@@ -147,46 +170,22 @@ static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDev
     for (int k = 0; k < CerbHandle::LANES; k++) CUDA_TRY(cudaEventCreate(&h->ev_lane[k]));
     for (int k = 0; k < CerbHandle::MAX_CHUNKS; k++) CUDA_TRY(cudaEventCreate(&h->ev_copy[k]));
     CUDA_TRY(cudaEventCreate(&h->ev0)); CUDA_TRY(cudaEventCreate(&h->ev1));
-    const size_t B = h->B, F = h->F, O = h->O;
+    const size_t F = h->F, O = h->O;
     h->ws_stride = ws_size(h->F);
-    CUDA_TRY(dmalloc(&h->d_rdesc, B)); CUDA_TRY(dmalloc(&h->d_rfeat, B * F)); CUDA_TRY(dmalloc(&h->d_robs, B * O)); CUDA_TRY(dmalloc(&h->d_rstate, B));
-    CUDA_TRY(dmalloc(&h->d_rpre, B * 10 * RAW_PRE_STRIDE)); CUDA_TRY(dmalloc(&h->d_rlam, B * F)); CUDA_TRY(dmalloc(&h->d_perm, B * F));
-    CUDA_TRY(dmalloc(&h->d_olam, B * F)); CUDA_TRY(dmalloc(&h->d_ostate, B * ST_STRIDE)); CUDA_TRY(dmalloc(&h->d_orep, B));
-    CUDA_TRY(dmalloc(&h->d_nfeat, B)); CUDA_TRY(dmalloc(&h->d_fstart, B * F)); CUDA_TRY(dmalloc(&h->d_fnobs, B * F)); CUDA_TRY(dmalloc(&h->d_foff, B * F));
-    CUDA_TRY(dmalloc(&h->d_flags, B)); CUDA_TRY(dmalloc(&h->d_stereo, B * O)); CUDA_TRY(dmalloc(&h->d_pmeta, B * PRIOR_META_STRIDE)); CUDA_TRY(dmalloc(&h->d_repi, B * 4));
-    CUDA_TRY(dmalloc(&h->d_obs, B * NOBS_PLANES * O)); CUDA_TRY(dmalloc(&h->d_pre, B * 10 * PRE_STRIDE)); CUDA_TRY(dmalloc(&h->d_sinfo, B * 10 * 961));
-    CUDA_TRY(dmalloc(&h->d_pJ, B * PRIOR_LD * PRIOR_LD)); CUDA_TRY(dmalloc(&h->d_pr, B * PRIOR_LD)); CUDA_TRY(dmalloc(&h->d_px0, B * 16 * 9)); CUDA_TRY(dmalloc(&h->d_pHp, B * PRIOR_LD * PRIOR_LD));
-    CUDA_TRY(dmalloc(&h->d_state, B * ST_STRIDE)); CUDA_TRY(dmalloc(&h->d_state0, B * ST_STRIDE)); CUDA_TRY(dmalloc(&h->d_lam, B * F)); CUDA_TRY(dmalloc(&h->d_lam0, B * F));
-    CUDA_TRY(dmalloc(&h->d_repd, B * 2)); CUDA_TRY(dmalloc(&h->d_ws, (size_t)CerbHandle::LANES * h->grid * h->ws_stride)); CUDA_TRY(dmalloc(&h->d_dbg, 2 * (NR + F) + 8)); CUDA_TRY(dmalloc(&h->d_G, 4));
-    CUDA_TRY(dmalloc(&h->d_probe_repi, 4)); CUDA_TRY(dmalloc(&h->d_probe_repd, 2));
-    CUDA_TRY(hmalloc(&h->h_rdesc, B)); CUDA_TRY(hmalloc(&h->h_rfeat, B * F)); CUDA_TRY(hmalloc(&h->h_robs, B * O)); CUDA_TRY(hmalloc(&h->h_rstate, B));
-    CUDA_TRY(hmalloc(&h->h_rpre, B * 10 * RAW_PRE_STRIDE)); CUDA_TRY(hmalloc(&h->h_rlam, B * F));
-    CUDA_TRY(hmalloc(&h->h_pJ, B * PRIOR_LD * PRIOR_LD)); CUDA_TRY(hmalloc(&h->h_pr, B * PRIOR_LD));
-    CUDA_TRY(hmalloc(&h->h_state, B * ST_STRIDE)); CUDA_TRY(hmalloc(&h->h_lam, B * F)); CUDA_TRY(hmalloc(&h->h_orep, B)); CUDA_TRY(hmalloc(&h->h_dbg, 2 * (NR + F) + 8));
-    h->nfeat.assign(B, 0); h->n0.assign(B, 0);
+    // the resident batch: elements per window, and whether the array has a pinned mirror
+    CUDA_TRY(alloc(h, h->rdesc, 1, true)); CUDA_TRY(alloc(h, h->rfeat, F, true)); CUDA_TRY(alloc(h, h->robs, O, true)); CUDA_TRY(alloc(h, h->rstate, 1, true));
+    CUDA_TRY(alloc(h, h->rpre, CERB_WINDOW_SIZE * RAW_PRE_STRIDE, true)); CUDA_TRY(alloc(h, h->rlam, F, true)); CUDA_TRY(alloc(h, h->perm, F));
+    CUDA_TRY(alloc(h, h->olam, F, true)); CUDA_TRY(alloc(h, h->ostate, ST_STRIDE, true)); CUDA_TRY(alloc(h, h->orep, 1, true));
+    CUDA_TRY(alloc(h, h->n_features, 1)); CUDA_TRY(alloc(h, h->feat_start, F)); CUDA_TRY(alloc(h, h->feat_nobs, F)); CUDA_TRY(alloc(h, h->feat_off, F));
+    CUDA_TRY(alloc(h, h->flags, 1)); CUDA_TRY(alloc(h, h->obs_stereo, O)); CUDA_TRY(alloc(h, h->prior_meta, PRIOR_META_STRIDE)); CUDA_TRY(alloc(h, h->rep_i, 4));
+    CUDA_TRY(alloc(h, h->obs, NOBS_PLANES * O)); CUDA_TRY(alloc(h, h->pre, CERB_WINDOW_SIZE * PRE_STRIDE)); CUDA_TRY(alloc(h, h->sinfo, CERB_WINDOW_SIZE * 961));
+    CUDA_TRY(alloc(h, h->prior_J, PRIOR_LD * PRIOR_LD, true)); CUDA_TRY(alloc(h, h->prior_r, PRIOR_LD, true)); CUDA_TRY(alloc(h, h->prior_x0, CERB_MAX_PRIOR_BLOCKS * 9));
+    CUDA_TRY(alloc(h, h->prior_Hp, PRIOR_LD * PRIOR_LD));
+    CUDA_TRY(alloc(h, h->state, ST_STRIDE)); CUDA_TRY(alloc(h, h->state0, ST_STRIDE)); CUDA_TRY(alloc(h, h->lam, F)); CUDA_TRY(alloc(h, h->lam0, F)); CUDA_TRY(alloc(h, h->rep_d, 2));
+    CUDA_TRY(dmalloc(h, &h->d_ws, (size_t)CerbHandle::LANES * h->grid * h->ws_stride)); CUDA_TRY(dmalloc(h, &h->d_dbg, 2 * (NR + F) + 8)); CUDA_TRY(dmalloc(h, &h->d_G, 4));
+    CUDA_TRY(dmalloc(h, &h->d_probe_repi, 4)); CUDA_TRY(dmalloc(h, &h->d_probe_repd, 2)); CUDA_TRY(hmalloc(h, &h->h_dbg, 2 * (NR + F) + 8));
+    h->nfeat.assign(h->B, 0); h->n0.assign(h->B, 0);
     CUDA_TRY(cudaMemcpy(h->d_G, cfg->g, 3 * sizeof(double), cudaMemcpyHostToDevice));
-#if !defined(CERB_CUSIM)
-    // The per-CTA workspace (W, the prior Hessian image: ~290 KB x one CTA per SM) is re-read every iteration while ~300 KB of inputs per
-    // window stream through once per linearisation; a persisting access-policy window on the compute stream can keep the workspace in L2.
-    // The solve is fp64-latency bound with DRAM nearly idle, so the carve-out mostly takes L2 away from the inputs: opt-in
-    // (CERB_L2_PERSIST=1), off by default.
-    {
-        const size_t ws_bytes = (size_t)h->grid * h->ws_stride * sizeof(double);
-        const size_t want = std::min<size_t>(ws_bytes, (size_t)prop.persistingL2CacheMaxSize);
-        if (want > 0 && std::getenv("CERB_L2_PERSIST") != nullptr) {
-            if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess) {
-                cudaStreamAttrValue av;
-                std::memset(&av, 0, sizeof(av));
-                av.accessPolicyWindow.base_ptr = h->d_ws;
-                av.accessPolicyWindow.num_bytes = std::min<size_t>(ws_bytes, (size_t)prop.accessPolicyMaxWindowSize);
-                av.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)want / (double)av.accessPolicyWindow.num_bytes);
-                av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-                av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-                if (cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &av) != cudaSuccess) cudaGetLastError();   // an optimisation only
-            } else cudaGetLastError();
-        }
-    }
-#endif
     return CERB_OK;
 }
 
@@ -196,14 +195,10 @@ void cerb_destroy(CerbHandle *h) {
     if (!h) return;
     cudaSetDevice(h->cfg.device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    void *dev[] = {h->d_rdesc, h->d_rfeat, h->d_robs, h->d_rstate, h->d_rpre, h->d_rlam, h->d_perm, h->d_olam, h->d_ostate, h->d_orep,
-                   h->d_nfeat, h->d_fstart, h->d_fnobs, h->d_foff, h->d_flags, h->d_stereo, h->d_pmeta, h->d_repi, h->d_obs, h->d_pre, h->d_sinfo, h->d_pJ, h->d_pr,
-                   h->d_px0, h->d_pHp, h->d_state, h->d_state0, h->d_lam, h->d_lam0, h->d_repd, h->d_ws, h->d_dbg, h->d_G, h->d_probe_repi, h->d_probe_repd};
-    for (void *p : dev) if (p) cudaFree(p);
+    for (void *p : h->dev_bufs) cudaFree(p);
     for (auto &c : h->arena) cudaFree(c.first);
     for (auto &r : h->regs) cudaHostUnregister((void *)r.first);
-    void *hst[] = {h->h_rdesc, h->h_rfeat, h->h_robs, h->h_rstate, h->h_rpre, h->h_rlam, h->h_pJ, h->h_pr, h->h_state, h->h_lam, h->h_orep, h->h_dbg};
-    for (void *p : hst) if (p) cudaFreeHost(p);
+    for (void *p : h->host_bufs) cudaFreeHost(p);
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int k = 0; k < CerbHandle::MAX_CHUNKS; k++) if (h->ev_copy[k]) cudaEventDestroy(h->ev_copy[k]);
@@ -231,10 +226,13 @@ static bool in_registered(const CerbHandle *h, const void *p, size_t bytes) {
     return false;
 }
 
-// One logical array of windows [w0, w0 + cn): window w holds `rows` rows of width_of(w) bytes, row r at src_of(w) + r * spitch;
-// device row (w - w0) * rows + r at dst + that * dpitch (stage: the pinned mirror of dst).
-template <class SrcOf, class WidthOf>
-static void plan_rows(const CerbHandle *h, UploadPlan &pl, int w0, int cn, char *dst, char *stage, size_t dpitch, int rows, size_t spitch, SrcOf src_of, WidthOf width_of) {
+// One logical array of windows [w0, w0 + cn): window w holds `rows` rows of width_of(w) bytes, row r at src_of(w) + r * spitch.  Each window's
+// slice of the resident array a is split into `rows` rows of equal pitch; the row lands `col` bytes into its device row (or, staged, into the
+// same place of the pinned mirror).
+template <class T, class SrcOf, class WidthOf>
+static void plan_rows(const CerbHandle *h, UploadPlan &pl, int w0, int cn, const Resident<T> &a, size_t col, int rows, size_t spitch, SrcOf src_of, WidthOf width_of) {
+    char *dst = (char *)a.at(w0) + col, *stage = (char *)a.h_at(w0) + col;
+    const size_t dpitch = a.per * sizeof(T) / rows;
     size_t maxw = 0; bool all_reg = true, uniform = true; int nact = 0;
     ptrdiff_t delta = 0;
     for (int i = 0; i < cn; i++) {
@@ -302,49 +300,53 @@ static int validate_window(const CerbHandle *h, const CerbWindowDesc &d, const C
     return validate_prior(d.prior);
 }
 
-static void run_stage_jobs(const std::vector<StageJob> &jobs) {
-    if (jobs.empty()) return;
-    size_t total = 0; for (const auto &j : jobs) total += j.bytes;
-    unsigned hw = std::thread::hardware_concurrency();
-    int nth = (int)std::min<unsigned>(hw ? hw : 1, 16u);
-    if (total < (4u << 20)) nth = 1;
-    auto work = [&](int t) { for (size_t k = t; k < jobs.size(); k += nth) std::memcpy(jobs[k].dst, jobs[k].src, jobs[k].bytes); };
+// fn(k) for k in [0, n), round robin over min(hardware threads, 16) host threads, or on the calling thread alone unless `wide`.  A thread stops
+// at its first failure (non-zero return); the first failing thread's code and message are returned.
+template <class Fn> static int fan_out(int n, bool wide, Fn fn) {
+    const unsigned hw = wide ? std::thread::hardware_concurrency() : 1;       // a system call: kept off the per-chunk path when nothing is staged
+    const int nth = (int)std::min<unsigned>(hw ? hw : 1, 16u);
+    std::vector<int> rcs(nth, CERB_OK); std::vector<std::string> errs(nth);
+    auto work = [&](int t) { for (int k = t; k < n; k += nth) { const int rc = fn(k); if (rc) { rcs[t] = rc; errs[t] = g_err; return; } } };
     std::vector<std::thread> th;
     for (int t = 1; t < nth; t++) th.emplace_back(work, t);
     work(0);
     for (auto &t : th) t.join();
+    for (int t = 0; t < nth; t++) if (rcs[t]) return fail(rcs[t], errs[t]);
+    return CERB_OK;
+}
+
+static void run_stage_jobs(const std::vector<StageJob> &jobs) {
+    if (jobs.empty()) return;
+    size_t total = 0; for (const auto &j : jobs) total += j.bytes;
+    fan_out((int)jobs.size(), total >= (4u << 20), [&](int k) { std::memcpy(jobs[k].dst, jobs[k].src, jobs[k].bytes); return (int)CERB_OK; });
 }
 
 // validate windows [w0, w0 + cn), move their raw descriptors to the device on stream s (staging only what is not registered)
 static int upload_raw(CerbHandle *h, int w0, int cn, const CerbWindowDesc *descs, const CerbWindowState *states, cudaStream_t s, double *t_stage_ms) {
     for (int w = w0; w < w0 + cn; w++) { int rc = validate_window(h, descs[w], states[w], &h->n0[w]); if (rc) return rc; h->nfeat[w] = descs[w].n_features; }
     UploadPlan pl;
-    const size_t F = h->F, O = h->O, W0 = (size_t)w0;
-    auto dv = [&](void *base, size_t per) { return (char *)base + W0 * per; };
-    plan_rows(h, pl, w0, cn, dv(h->d_rdesc, sizeof(CerbWindowDesc)), dv(h->h_rdesc, sizeof(CerbWindowDesc)), sizeof(CerbWindowDesc), 1, 0,
-              [&](int w) { return (const void *)&descs[w]; }, [&](int) { return sizeof(CerbWindowDesc); });
-    plan_rows(h, pl, w0, cn, dv(h->d_rstate, sizeof(CerbWindowState)), dv(h->h_rstate, sizeof(CerbWindowState)), sizeof(CerbWindowState), 1, 0,
-              [&](int w) { return (const void *)&states[w]; }, [&](int) { return sizeof(CerbWindowState); });
-    plan_rows(h, pl, w0, cn, dv(h->d_rfeat, F * sizeof(CerbFeature)), dv(h->h_rfeat, F * sizeof(CerbFeature)), F * sizeof(CerbFeature), 1, 0,
+    plan_rows(h, pl, w0, cn, h->rdesc, 0, 1, 0, [&](int w) { return (const void *)&descs[w]; }, [&](int) { return sizeof(CerbWindowDesc); });
+    plan_rows(h, pl, w0, cn, h->rstate, 0, 1, 0, [&](int w) { return (const void *)&states[w]; }, [&](int) { return sizeof(CerbWindowState); });
+    plan_rows(h, pl, w0, cn, h->rfeat, 0, 1, 0,
               [&](int w) { return (const void *)descs[w].features; }, [&](int w) { return (size_t)descs[w].n_features * sizeof(CerbFeature); });
-    plan_rows(h, pl, w0, cn, dv(h->d_robs, O * sizeof(CerbObservation)), dv(h->h_robs, O * sizeof(CerbObservation)), O * sizeof(CerbObservation), 1, 0,
+    plan_rows(h, pl, w0, cn, h->robs, 0, 1, 0,
               [&](int w) { return (const void *)descs[w].obs; }, [&](int w) { return (size_t)descs[w].n_obs * sizeof(CerbObservation); });
-    plan_rows(h, pl, w0, cn, dv(h->d_rlam, F * 8), dv(h->h_rlam, F * 8), F * 8, 1, 0,
+    plan_rows(h, pl, w0, cn, h->rlam, 0, 1, 0,
               [&](int w) { return (const void *)states[w].para_Feature; }, [&](int w) { return (size_t)descs[w].n_features * 8; });
-    // preintegration results: the members IMULegFactor::Evaluate reads -- head (33 doubles) and, contiguous in the struct, jacobian columns 21..30 + covariance
-    const size_t pre_pitch = (size_t)RAW_PRE_STRIDE * 8, tail_off = (size_t)(RAW_PRE_HEAD + RAW_PRE_JCOL0 * 31) * 8, tail_w = sizeof(CerbIMULegPreint) - tail_off;
+    // preintegration results, one row per factor: the members IMULegFactor::Evaluate reads -- head (33 doubles) and, contiguous in the struct,
+    // jacobian columns 21..30 + covariance
+    const size_t tail_off = (size_t)(RAW_PRE_HEAD + RAW_PRE_JCOL0 * 31) * 8, tail_w = sizeof(CerbIMULegPreint) - tail_off;
     static_assert(sizeof(CerbIMULegPreint) == (33 + 2 * 961) * 8, "CerbIMULegPreint layout");
     static_assert(sizeof(CerbIMUPreint) == 467 * 8 && sizeof(CerbIMUPreint) <= RAW_PRE_STRIDE * 8, "CerbIMUPreint layout");
-    plan_rows(h, pl, w0, cn, dv(h->d_rpre, 10 * pre_pitch), dv(h->h_rpre, 10 * pre_pitch), pre_pitch, CERB_WINDOW_SIZE, sizeof(CerbIMULegPreint),
+    plan_rows(h, pl, w0, cn, h->rpre, 0, CERB_WINDOW_SIZE, sizeof(CerbIMULegPreint),
               [&](int w) { return (const void *)descs[w].preint; }, [&](int w) { return descs[w].preint ? (size_t)RAW_PRE_HEAD * 8 : (size_t)0; });
-    plan_rows(h, pl, w0, cn, dv(h->d_rpre, 10 * pre_pitch) + RAW_PRE_HEAD * 8, dv(h->h_rpre, 10 * pre_pitch) + RAW_PRE_HEAD * 8, pre_pitch, CERB_WINDOW_SIZE, sizeof(CerbIMULegPreint),
+    plan_rows(h, pl, w0, cn, h->rpre, RAW_PRE_HEAD * 8, CERB_WINDOW_SIZE, sizeof(CerbIMULegPreint),
               [&](int w) { return (const void *)((const char *)descs[w].preint + tail_off); }, [&](int w) { return descs[w].preint ? tail_w : (size_t)0; });
-    plan_rows(h, pl, w0, cn, dv(h->d_rpre, 10 * pre_pitch), dv(h->h_rpre, 10 * pre_pitch), pre_pitch, CERB_WINDOW_SIZE, sizeof(CerbIMUPreint),
+    plan_rows(h, pl, w0, cn, h->rpre, 0, CERB_WINDOW_SIZE, sizeof(CerbIMUPreint),
               [&](int w) { return (const void *)descs[w].imu_preint; }, [&](int w) { return descs[w].preint ? (size_t)0 : sizeof(CerbIMUPreint); });
-    const size_t pj_pitch = (size_t)PRIOR_LD * PRIOR_LD * 8;
-    plan_rows(h, pl, w0, cn, dv(h->d_pJ, pj_pitch), dv(h->h_pJ, pj_pitch), pj_pitch, 1, 0,
+    plan_rows(h, pl, w0, cn, h->prior_J, 0, 1, 0,
               [&](int w) { return (const void *)descs[w].prior.linearized_jacobians; }, [&](int w) { return descs[w].prior.valid ? (size_t)descs[w].prior.n * descs[w].prior.n * 8 : (size_t)0; });
-    plan_rows(h, pl, w0, cn, dv(h->d_pr, PRIOR_LD * 8), dv(h->h_pr, PRIOR_LD * 8), (size_t)PRIOR_LD * 8, 1, 0,
+    plan_rows(h, pl, w0, cn, h->prior_r, 0, 1, 0,
               [&](int w) { return (const void *)descs[w].prior.linearized_residuals; }, [&](int w) { return descs[w].prior.valid ? (size_t)descs[w].prior.n * 8 : (size_t)0; });
     const auto t0 = std::chrono::steady_clock::now();
     run_stage_jobs(pl.stage);
@@ -360,12 +362,11 @@ static int upload_raw(CerbHandle *h, int w0, int cn, const CerbWindowDesc *descs
 // device pack of windows [w0, w0 + cn) (after their raw descriptors have arrived) on stream s
 static int enqueue_pack(CerbHandle *h, int w0, int cn, cudaStream_t s) {
     PackParams P;
-    const size_t W0 = (size_t)w0, F = h->F, O = h->O;
     P.n = cn; P.maxF = h->F; P.maxObs = h->O;
-    P.rdesc = h->d_rdesc + W0; P.rfeat = h->d_rfeat + W0 * F; P.robs = h->d_robs + W0 * O; P.rpre = h->d_rpre + W0 * 10 * RAW_PRE_STRIDE; P.rstate = h->d_rstate + W0; P.rlam = h->d_rlam + W0 * F;
-    P.n_features = h->d_nfeat + W0; P.feat_start = h->d_fstart + W0 * F; P.feat_nobs = h->d_fnobs + W0 * F; P.feat_off = h->d_foff + W0 * F; P.flags = h->d_flags + W0;
-    P.obs_stereo = h->d_stereo + W0 * O; P.prior_meta = h->d_pmeta + W0 * PRIOR_META_STRIDE; P.perm = h->d_perm + W0 * F;
-    P.obs = h->d_obs + W0 * NOBS_PLANES * O; P.pre = h->d_pre + W0 * 10 * PRE_STRIDE; P.prior_x0 = h->d_px0 + W0 * 16 * 9; P.state0 = h->d_state0 + W0 * ST_STRIDE; P.lam0 = h->d_lam0 + W0 * F;
+    P.rdesc = h->rdesc.at(w0); P.rfeat = h->rfeat.at(w0); P.robs = h->robs.at(w0); P.rpre = h->rpre.at(w0); P.rstate = h->rstate.at(w0); P.rlam = h->rlam.at(w0);
+    P.n_features = h->n_features.at(w0); P.feat_start = h->feat_start.at(w0); P.feat_nobs = h->feat_nobs.at(w0); P.feat_off = h->feat_off.at(w0); P.flags = h->flags.at(w0);
+    P.obs_stereo = h->obs_stereo.at(w0); P.prior_meta = h->prior_meta.at(w0); P.perm = h->perm.at(w0);
+    P.obs = h->obs.at(w0); P.pre = h->pre.at(w0); P.prior_x0 = h->prior_x0.at(w0); P.state0 = h->state0.at(w0); P.lam0 = h->lam0.at(w0);
     CERB_LAUNCH(pack_kernel, std::min(cn, 8 * h->sm_count), PACK_THREADS, 0, s, P);
     CUDA_TRY(cudaGetLastError());
     return CERB_OK;
@@ -380,8 +381,8 @@ static int upload(CerbHandle *h, int n, const CerbWindowDesc *descs, const CerbW
 // device slot -> caller's feature index of the resident batch (computed by the pack kernel; fetched on demand by the probes / feature passes)
 static int ensure_perm(CerbHandle *h) {
     if (h->perm_valid) return CERB_OK;
-    h->h_perm.resize((size_t)h->B * h->F);
-    CUDA_TRY(cudaMemcpyAsync(h->h_perm.data(), h->d_perm, (size_t)h->n * h->F * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    h->h_perm.resize((size_t)h->B * h->perm.per);
+    CUDA_TRY(cudaMemcpyAsync(h->h_perm.data(), h->perm.d, h->perm.bytes(h->n), cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(cudaStreamSynchronize(h->stream));
     h->perm_valid = true;
     return CERB_OK;
@@ -396,29 +397,31 @@ static SolveParams make_params(CerbHandle *h, int w0, int n, int max_iters, doub
     P.sqrt_info = c.visual_sqrt_info; P.huber = c.huber_delta;
     P.radius0 = c.initial_trust_region_radius; P.max_radius = c.max_trust_region_radius; P.min_radius = c.min_trust_region_radius;
     P.min_rel_dec = c.min_relative_decrease; P.ftol = c.function_tolerance; P.gtol = c.gradient_tolerance; P.ptol = c.parameter_tolerance;
-    const size_t W0 = (size_t)w0, F = h->F, O = h->O;
-    P.n_features = h->d_nfeat + W0; P.feat_start = h->d_fstart + W0 * F; P.feat_nobs = h->d_fnobs + W0 * F; P.feat_off = h->d_foff + W0 * F; P.flags = h->d_flags + W0;
-    P.obs = h->d_obs + W0 * NOBS_PLANES * O; P.obs_stereo = h->d_stereo + W0 * O; P.pre = h->d_pre + W0 * 10 * PRE_STRIDE; P.sinfo = h->d_sinfo + W0 * 10 * 961;
-    P.prior_J = h->d_pJ + W0 * PRIOR_LD * PRIOR_LD; P.prior_r = h->d_pr + W0 * PRIOR_LD; P.prior_x0 = h->d_px0 + W0 * 16 * 9; P.prior_Hp = h->d_pHp + W0 * PRIOR_LD * PRIOR_LD;
-    P.prior_meta = h->d_pmeta + W0 * PRIOR_META_STRIDE;
-    P.state = h->d_state + W0 * ST_STRIDE; P.lam = h->d_lam + W0 * F; P.rep_i = h->d_repi + W0 * 4; P.rep_d = h->d_repd + W0 * 2; P.ws = h->d_ws; P.ws_stride = h->ws_stride;
+    P.n_features = h->n_features.at(w0); P.feat_start = h->feat_start.at(w0); P.feat_nobs = h->feat_nobs.at(w0); P.feat_off = h->feat_off.at(w0); P.flags = h->flags.at(w0);
+    P.obs = h->obs.at(w0); P.obs_stereo = h->obs_stereo.at(w0); P.pre = h->pre.at(w0); P.sinfo = h->sinfo.at(w0);
+    P.prior_J = h->prior_J.at(w0); P.prior_r = h->prior_r.at(w0); P.prior_x0 = h->prior_x0.at(w0); P.prior_Hp = h->prior_Hp.at(w0); P.prior_meta = h->prior_meta.at(w0);
+    P.state = h->state.at(w0); P.lam = h->lam.at(w0); P.rep_i = h->rep_i.at(w0); P.rep_d = h->rep_d.at(w0); P.ws = h->d_ws; P.ws_stride = h->ws_stride;
     P.dbg = dbg; P.dbg_window = dbg_window;
     P.test_fail_factorizations = h->test_fail_factorizations; P.test_initial_mu = h->test_initial_mu;
     P.no_bulk_copy = std::getenv("CERB_NO_TMA") != nullptr;
     return P;
 }
 
+// sqrt_info of the IMU-leg factors and the Gram matrix of the prior of windows [w0, w0 + n), on stream s
+static void enqueue_prepare(CerbHandle *h, int w0, int n, cudaStream_t s) {
+    const int nfac = n * CERB_WINDOW_SIZE;
+    CERB_LAUNCH(imu_leg_prepare_kernel, (nfac + 1) / 2, 64, 0, s, nfac, (const double *)h->pre.at(w0), h->sinfo.at(w0));
+    CERB_LAUNCH(prior_prepare_kernel, n, 256, (size_t)PRIOR_TROWS * PRIOR_TLD * sizeof(double), s, (const double *)h->prior_J.at(w0), (const int *)h->prior_meta.at(w0), h->prior_Hp.at(w0));
+}
+
 // restore the initial states of windows [w0, w0 + n), prepare (sqrt_info, prior Gram matrix) and solve; asynchronous on the stream
 static int enqueue_solve(CerbHandle *h, int w0, int n, int max_iters, double *dbg, int dbg_window, bool restore = true, bool probe = false, int lane = 0) {
     cudaStream_t s = h->lane[lane];
-    const size_t W0 = (size_t)w0;
     if (restore) {
-        CUDA_TRY(cudaMemcpyAsync(h->d_state + W0 * ST_STRIDE, h->d_state0 + W0 * ST_STRIDE, (size_t)n * ST_STRIDE * sizeof(double), cudaMemcpyDeviceToDevice, s));
-        CUDA_TRY(cudaMemcpyAsync(h->d_lam + W0 * h->F, h->d_lam0 + W0 * h->F, (size_t)n * h->F * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(h->state.at(w0), h->state0.at(w0), h->state.bytes(n), cudaMemcpyDeviceToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(h->lam.at(w0), h->lam0.at(w0), h->lam.bytes(n), cudaMemcpyDeviceToDevice, s));
     }
-    const int nfac = n * 10;
-    CERB_LAUNCH(imu_leg_prepare_kernel, (nfac + 1) / 2, 64, 0, s, nfac, (const double *)(h->d_pre + W0 * 10 * PRE_STRIDE), h->d_sinfo + W0 * 10 * 961);
-    CERB_LAUNCH(prior_prepare_kernel, n, 256, (size_t)PRIOR_TROWS * PRIOR_TLD * sizeof(double), s, (const double *)(h->d_pJ + W0 * PRIOR_LD * PRIOR_LD), (const int *)(h->d_pmeta + W0 * PRIOR_META_STRIDE), h->d_pHp + W0 * PRIOR_LD * PRIOR_LD);
+    enqueue_prepare(h, w0, n, s);
     SolveParams P = make_params(h, w0, n, max_iters, dbg, dbg_window);
     P.ws = h->d_ws + (size_t)lane * h->grid * h->ws_stride;                      // kernels of different lanes run concurrently: one workspace slice each
     if (probe) { P.rep_i = h->d_probe_repi; P.rep_d = h->d_probe_repd; }       // a probe leaves the reports of the batch alone
@@ -445,28 +448,34 @@ static int collect_time(CerbHandle *h) {
     return CERB_OK;
 }
 
+// a batch of states in device layout: state [n][ST_STRIDE], lam [n][F] in device feature order
+struct States { Resident<double> state, lam; };
+// the current states of the resident batch: the solved ones after a solve, else the uploaded (or cerb_batch_update_states') initial ones
+static States resident_states(const CerbHandle *h) { return h->solved ? States{h->state, h->lam} : States{h->state0, h->lam0}; }
+
 static int download(CerbHandle *h, CerbWindowState *states, CerbSolveReport *reports) {
-    const int n = h->n; const size_t F = h->F;
+    const int n = h->n;
     cudaStream_t s = h->stream;
+    const States cur = resident_states(h);
     UnpackParams U;
-    U.n = n; U.maxF = h->F; U.n_features = h->d_nfeat; U.perm = h->d_perm; U.rep_i = h->d_repi; U.rep_d = h->d_repd;
-    U.lam = h->solved ? h->d_lam : h->d_lam0; U.state = h->solved ? h->d_state : h->d_state0;
-    U.olam = h->d_olam; U.orep = h->d_orep; U.ostate = h->d_ostate;
+    U.n = n; U.maxF = h->F; U.n_features = h->n_features.d; U.perm = h->perm.d; U.rep_i = h->rep_i.d; U.rep_d = h->rep_d.d;
+    U.lam = cur.lam.d; U.state = cur.state.d;
+    U.olam = h->olam.d; U.orep = h->orep.d; U.ostate = h->ostate.d;
     CERB_LAUNCH(unpack_kernel, std::min(n, 8 * h->sm_count), PACK_THREADS, 0, s, U);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(h->h_state, h->d_ostate, (size_t)n * ST_STRIDE * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(h->h_lam, h->d_olam, n * F * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(h->h_orep, h->d_orep, (size_t)n * sizeof(CerbSolveReport), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(h->ostate.h, h->ostate.d, h->ostate.bytes(n), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(h->olam.h, h->olam.d, h->olam.bytes(n), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(h->orep.h, h->orep.d, h->orep.bytes(n), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     int rc = collect_time(h); if (rc) return rc;
     int status = CERB_OK;
     for (int w = 0; w < n; w++) {
         if (states) {
-            std::memcpy(&states[w], h->h_state + (size_t)w * ST_STRIDE, ST_SIZE * sizeof(double));        // para_Pose .. para_Td: contiguous, same order
-            if (states[w].para_Feature && h->nfeat[w]) std::memcpy(states[w].para_Feature, h->h_lam + (size_t)w * F, (size_t)h->nfeat[w] * sizeof(double));
+            std::memcpy(&states[w], h->ostate.h_at(w), ST_SIZE * sizeof(double));        // para_Pose .. para_Td: contiguous, same order
+            if (states[w].para_Feature && h->nfeat[w]) std::memcpy(states[w].para_Feature, h->olam.h_at(w), (size_t)h->nfeat[w] * sizeof(double));
         }
-        if (reports) reports[w] = h->h_orep[w];
-        if (h->h_orep[w].status != 0) status = CERB_ERR_NON_FINITE;
+        if (reports) reports[w] = h->orep.h[w];
+        if (h->orep.h[w].status != 0) status = CERB_ERR_NON_FINITE;
     }
     if (status) return fail(status, "at least one window produced a non-finite cost (see reports[].status)");
     return CERB_OK;
@@ -664,18 +673,25 @@ static void pack_imu_preint(const CerbIMUPreint &p, double *o) {
     for (int k = 0; k < PRE_STRIDE; k++) o[k] = pack_pre_imu(raw, k);
 }
 static const int kImuTo31[15] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 21, 22, 23, 24, 25, 26};
-static int pack_prior(const CerbPrior &pr, int *meta, double *J, double *r, double *x0) {
+// the prior's record on the device apart from its matrix and residuals: meta (PRIOR_META_STRIDE ints: valid, n, num_blocks, -, then kind /
+// index / column of block b at 4 + 3 b) and x0 (9 doubles per block)
+static void encode_prior(const CerbPrior &pr, int *meta, double *x0) {
     std::memset(meta, 0, PRIOR_META_STRIDE * sizeof(int));
-    if (!pr.valid) return CERB_OK;
-    int rc = validate_prior(pr); if (rc) return rc;
+    if (!pr.valid) return;
     meta[0] = 1; meta[1] = pr.n; meta[2] = pr.num_blocks;
     for (int b = 0; b < pr.num_blocks; b++) {
         meta[4 + 3 * b] = pr.block_kind[b]; meta[5 + 3 * b] = pr.block_index[b]; meta[6 + 3 * b] = pr.block_col[b];
         for (int k = 0; k < 9; k++) x0[9 * b + k] = pr.block_x0[b][k];
     }
-    std::memcpy(J, pr.linearized_jacobians, sizeof(double) * pr.n * pr.n);
-    std::memcpy(r, pr.linearized_residuals, sizeof(double) * pr.n);
-    return CERB_OK;
+}
+static void decode_prior(const int *meta, const double *x0, CerbPrior &pr) {
+    pr.valid = 0; pr.n = 0; pr.num_blocks = 0;
+    if (!meta[0]) return;
+    pr.valid = 1; pr.n = meta[1]; pr.num_blocks = meta[2];
+    for (int b = 0; b < pr.num_blocks; b++) {
+        pr.block_kind[b] = meta[4 + 3 * b]; pr.block_index[b] = meta[5 + 3 * b]; pr.block_col[b] = meta[6 + 3 * b];
+        for (int k = 0; k < 9; k++) pr.block_x0[b][k] = x0[9 * b + k];
+    }
 }
 
 
@@ -704,13 +720,11 @@ int cerb_eval_projection(CerbHandle *h, int32_t kind, int32_t n, const double *p
     return CERB_OK;
 }
 
-int cerb_eval_imu_leg(CerbHandle *h, int32_t n, const CerbIMULegPreint *preint, const double *params, double *residuals, double *jacobians, double *sqrt_info) {
-    if (!h || n < 1 || !preint || !params) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_eval_imu_leg: bad argument");
-    CERB_DEVICE(h);
+// IMU-leg factors of n packed preintegration records (PRE_STRIDE each) and parameter rows (40 each): residuals [n][31], Jacobians [n][31 x 40]
+// and sqrt_info [n][961] into the host arrays that are not null
+static int eval_imu_leg_packed(CerbHandle *h, int n, const double *packed, const double *params, double *residuals, double *jacobians, double *sqrt_info) {
     cudaStream_t s = h->stream; DevBuf B(h); const size_t N = n;
-    std::vector<double> packed(N * PRE_STRIDE, 0.0);
-    for (int k = 0; k < n; k++) pack_preint(preint[k], packed.data() + (size_t)k * PRE_STRIDE);
-    double *dpre = B.up(packed.data(), N * PRE_STRIDE, s), *dsi = B.up(nullptr, N * 961, s), *dpar = B.up(params, 40 * N, s);
+    double *dpre = B.up(packed, N * PRE_STRIDE, s), *dsi = B.up(nullptr, N * 961, s), *dpar = B.up(params, 40 * N, s);
     double *dr = B.up(nullptr, 31 * N, s), *dJ = jacobians ? B.up(nullptr, 31 * 40 * N, s) : nullptr;
     if (!dpre || !dsi || !dpar || !dr) return fail(CERB_ERR_CUDA, "device allocation failed");
     CERB_LAUNCH(imu_leg_prepare_kernel, (n + 1) / 2, 64, 0, s, (int)n, (const double *)dpre, dsi);
@@ -723,27 +737,26 @@ int cerb_eval_imu_leg(CerbHandle *h, int32_t n, const CerbIMULegPreint *preint, 
     return CERB_OK;
 }
 
+int cerb_eval_imu_leg(CerbHandle *h, int32_t n, const CerbIMULegPreint *preint, const double *params, double *residuals, double *jacobians, double *sqrt_info) {
+    if (!h || n < 1 || !preint || !params) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_eval_imu_leg: bad argument");
+    CERB_DEVICE(h);
+    std::vector<double> packed((size_t)n * PRE_STRIDE, 0.0);
+    for (int k = 0; k < n; k++) pack_preint(preint[k], packed.data() + (size_t)k * PRE_STRIDE);
+    return eval_imu_leg_packed(h, n, packed.data(), params, residuals, jacobians, sqrt_info);
+}
+
 int cerb_eval_imu(CerbHandle *h, int32_t n, const CerbIMUPreint *preint, const double *params, double *residuals, double *jacobians, double *sqrt_info) {
     if (!h || n < 1 || !preint || !params) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_eval_imu: bad argument");
     CERB_DEVICE(h);
-    cudaStream_t s = h->stream; DevBuf B(h); const size_t N = n;
+    const size_t N = n;
     std::vector<double> packed(N * PRE_STRIDE), p40(N * 40, 0.0);
     for (int k = 0; k < n; k++) {
         pack_imu_preint(preint[k], packed.data() + (size_t)k * PRE_STRIDE);
         const double *q = params + (size_t)k * 32; double *o = p40.data() + (size_t)k * 40;
         std::memcpy(o, q, 16 * sizeof(double)); std::memcpy(o + 20, q + 16, 16 * sizeof(double));     // leg-bias slots stay 0
     }
-    double *dpre = B.up(packed.data(), N * PRE_STRIDE, s), *dsi = B.up(nullptr, N * 961, s), *dpar = B.up(p40.data(), 40 * N, s);
-    double *dr = B.up(nullptr, 31 * N, s), *dJ = jacobians ? B.up(nullptr, 31 * 40 * N, s) : nullptr;
-    if (!dpre || !dsi || !dpar || !dr) return fail(CERB_ERR_CUDA, "device allocation failed");
-    CERB_LAUNCH(imu_leg_prepare_kernel, (n + 1) / 2, 64, 0, s, (int)n, (const double *)dpre, dsi);
-    CERB_LAUNCH(imu_leg_eval_kernel, n, 128, 0, s, (int)n, (const double *)dpre, (const double *)dsi, (const double *)dpar, (const double *)h->d_G, dr, dJ);
-    CUDA_TRY(cudaGetLastError());
     std::vector<double> hr(31 * N), hj(jacobians ? 31 * 40 * N : 0), hs(961 * N);
-    CUDA_TRY(cudaMemcpyAsync(hr.data(), dr, hr.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    if (jacobians) CUDA_TRY(cudaMemcpyAsync(hj.data(), dJ, hj.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hs.data(), dsi, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
+    int rc = eval_imu_leg_packed(h, n, packed.data(), p40.data(), hr.data(), jacobians ? hj.data() : nullptr, hs.data()); if (rc) return rc;
     // gather the 15 rows P, R, V, BA, BG and the blocks pose_i, speedbias_i, pose_j, speedbias_j
     const int boff31[4] = {0, 7, 20, 27}, bsz[4] = {7, 9, 7, 9}, boff15[4] = {0, 7, 16, 23};
     for (int k = 0; k < n; k++) {
@@ -762,7 +775,10 @@ int cerb_eval_prior(CerbHandle *h, const CerbPrior *prior, const CerbWindowState
     if (!h || !prior || !state || !prior->valid || !residuals) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_eval_prior: bad argument");
     CERB_DEVICE(h);
     std::vector<int> meta(PRIOR_META_STRIDE); std::vector<double> J(PRIOR_LD * PRIOR_LD, 0.0), r(PRIOR_LD, 0.0), x0(16 * 9, 0.0), st(ST_STRIDE, 0.0);
-    int rc = pack_prior(*prior, meta.data(), J.data(), r.data(), x0.data()); if (rc) return rc;
+    int rc = validate_prior(*prior); if (rc) return rc;
+    encode_prior(*prior, meta.data(), x0.data());
+    std::memcpy(J.data(), prior->linearized_jacobians, sizeof(double) * prior->n * prior->n);
+    std::memcpy(r.data(), prior->linearized_residuals, sizeof(double) * prior->n);
     std::memcpy(st.data() + ST_POSE, state->para_Pose, sizeof(state->para_Pose)); std::memcpy(st.data() + ST_SB, state->para_SpeedBias, sizeof(state->para_SpeedBias));
     std::memcpy(st.data() + ST_LB, state->para_LegBias, sizeof(state->para_LegBias)); std::memcpy(st.data() + ST_EX, state->para_Ex_Pose, sizeof(state->para_Ex_Pose));
     st[ST_TD] = state->para_Td[0];
@@ -800,37 +816,53 @@ int cerb_a1_kinematics(CerbHandle *h, int32_t n, const double *q, const double *
 }
 
 // ---- per-feature steps on the resident batch ------------------------------------------------------------------------
-static int feature_pass(CerbHandle *h, int which, double param, double *out, int32_t *remove) {
-    if (!h || !out) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
+// One pass over the features of the resident batch at its current states: launch(s, blocks, threads, states, out) enqueues the pass kernel,
+// which writes `planes` planes of [n][F] doubles in device slot order.  They come back in the caller's feature order: store(q, v, N) is called
+// for entry q = w * F + f of the first nfeat[w] features of each window w (plane p at v[p * N + q]).  The caller's entries past nfeat[w] are
+// left as they are.
+}  // extern "C"
+template <class Launch, class Store> static int feature_pass(CerbHandle *h, int planes, Launch launch, Store store) {
     CERB_DEVICE(h);
     if (h->n < 1) return fail(CERB_ERR_BAD_ARGUMENT, "no resident batch");
     const int n = h->n, F = h->F;
+    const size_t N = (size_t)n * F;
     cudaStream_t s = h->stream; DevBuf B(h);
-    double *d_out = B.up(nullptr, (size_t)n * F, s), *d_perm_out = B.up(nullptr, (size_t)n * F, s);
+    double *d_out = B.up(nullptr, planes * N, s), *d_perm_out = B.up(nullptr, planes * N, s);
     if (!d_out || !d_perm_out) return fail(CERB_ERR_CUDA, "device allocation failed");
-    const int threads = 128, blocks = (n * F + threads - 1) / threads;
-    const double *d_st = h->solved ? h->d_state : h->d_state0, *d_lm = h->solved ? h->d_lam : h->d_lam0;
-    if (which == 0)
-        CERB_LAUNCH(outlier_error_kernel, blocks, threads, 0, s, n, F, h->O, (const int *)h->d_nfeat, (const int *)h->d_fstart, (const int *)h->d_fnobs, (const int *)h->d_foff,
-                    (const double *)h->d_obs, (const int *)h->d_stereo, d_st, d_lm, d_out);
-    else
-        CERB_LAUNCH(triangulate_kernel, blocks, threads, 0, s, n, F, h->O, (const int *)h->d_nfeat, (const int *)h->d_fstart, (const int *)h->d_fnobs, (const int *)h->d_foff,
-                    (const double *)h->d_obs, (const int *)h->d_stereo, d_st, d_lm, param, d_out);
-    CERB_LAUNCH(unpermute_kernel, blocks, threads, 0, s, n, F, 1, (const int *)h->d_nfeat, (const int *)h->d_perm, (const double *)d_out, d_perm_out);      // device slot -> caller's feature index
+    const int threads = 128, blocks = (int)((N + threads - 1) / threads);
+    launch(s, blocks, threads, resident_states(h), d_out);
+    CERB_LAUNCH(unpermute_kernel, blocks, threads, 0, s, n, F, planes, (const int *)h->n_features.d, (const int *)h->perm.d, (const double *)d_out, d_perm_out);   // device slot -> caller's feature index
     CUDA_TRY(cudaGetLastError());
-    std::vector<double> tmp((size_t)n * F);
+    std::vector<double> tmp(planes * N);
     CUDA_TRY(cudaMemcpyAsync(tmp.data(), d_perm_out, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     for (int w = 0; w < n; w++)
-        for (int f = 0; f < h->nfeat[w]; f++) {
-            const double v = tmp[(size_t)w * F + f];
-            out[(size_t)w * F + f] = v;
-            if (remove) remove[(size_t)w * F + f] = (v * param > 3.0) ? 1 : 0;
-        }
+        for (int f = 0; f < h->nfeat[w]; f++) store((size_t)w * F + f, tmp.data(), N);
     return CERB_OK;
 }
-int cerb_batch_outlier_errors(CerbHandle *h, double focal_length, double *ave_err, int32_t *remove) { return feature_pass(h, 0, focal_length, ave_err, remove); }
-int cerb_batch_triangulate(CerbHandle *h, double init_depth, double *depth) { return feature_pass(h, 1, init_depth, depth, nullptr); }
+extern "C" {
+
+int cerb_batch_outlier_errors(CerbHandle *h, double focal_length, double *ave_err, int32_t *remove) {
+    if (!h || !ave_err) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
+    return feature_pass(h, 1, [&](cudaStream_t s, int blocks, int threads, const States &cur, double *out) {
+        CERB_LAUNCH(outlier_error_kernel, blocks, threads, 0, s, h->n, h->F, h->O, (const int *)h->n_features.d, (const int *)h->feat_start.d, (const int *)h->feat_nobs.d,
+                    (const int *)h->feat_off.d, (const double *)h->obs.d, (const int *)h->obs_stereo.d, (const double *)cur.state.d, (const double *)cur.lam.d, out);
+    }, [&](size_t q, const double *v, size_t) { ave_err[q] = v[q]; if (remove) remove[q] = (v[q] * focal_length > 3.0) ? 1 : 0; });
+}
+int cerb_batch_triangulate(CerbHandle *h, double init_depth, double *depth) {
+    if (!h || !depth) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
+    return feature_pass(h, 1, [&](cudaStream_t s, int blocks, int threads, const States &cur, double *out) {
+        CERB_LAUNCH(triangulate_kernel, blocks, threads, 0, s, h->n, h->F, h->O, (const int *)h->n_features.d, (const int *)h->feat_start.d, (const int *)h->feat_nobs.d,
+                    (const int *)h->feat_off.d, (const double *)h->obs.d, (const int *)h->obs_stereo.d, (const double *)cur.state.d, (const double *)cur.lam.d, init_depth, out);
+    }, [&](size_t q, const double *v, size_t) { depth[q] = v[q]; });
+}
+int cerb_batch_shift_depth(CerbHandle *h, double init_depth, int32_t *new_start_frame, double *depth, int32_t *keep) {
+    if (!h || !new_start_frame || !depth || !keep) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
+    return feature_pass(h, 3, [&](cudaStream_t s, int blocks, int threads, const States &cur, double *out) {
+        CERB_LAUNCH(shift_depth_kernel, blocks, threads, 0, s, h->n, h->F, h->O, (const int *)h->n_features.d, (const int *)h->feat_start.d, (const int *)h->feat_nobs.d,
+                    (const int *)h->feat_off.d, (const double *)h->obs.d, (const double *)cur.state.d, (const double *)cur.lam.d, init_depth, out);
+    }, [&](size_t q, const double *v, size_t N) { new_start_frame[q] = (int32_t)v[q]; depth[q] = v[N + q]; keep[q] = (int32_t)v[2 * N + q]; });
+}
 // test hook: CERB_TEST_MARG_SMEM=<bytes> shrinks the shared-memory budget of the eigen-solver's memory plan (split / global layouts on small matrices)
 static size_t marg_smem_limit() {
     const char *e = std::getenv("CERB_TEST_MARG_SMEM");
@@ -869,10 +901,33 @@ CERB_GLOBAL void permute_lam_kernel(int n, int F, const int *n_features, const i
     if (k < n_features[w]) lam_dev[idx] = lam_caller[(size_t)w * F + perm[idx]];
 }
 
+// The caller's states of the resident batch into dst: para_Pose .. para_Td as they are, para_Feature in device feature order.  `who` names the
+// entry point in the error messages.  hst receives the host image of dst.state; the copies are done when this returns.
+static int states_to_device(CerbHandle *h, DevBuf &B, const CerbWindowState *states, const char *who, const States &dst, std::vector<double> &hst) {
+    const int n = h->n, F = h->F;
+    cudaStream_t s = h->stream;
+    hst.assign(n * dst.state.per, 0.0);
+    std::vector<double> hl(n * dst.lam.per, 0.0);
+    for (int w = 0; w < n; w++) {
+        std::memcpy(hst.data() + w * dst.state.per, &states[w], ST_SIZE * sizeof(double));
+        if (h->nfeat[w]) {
+            if (!states[w].para_Feature) return fail(CERB_ERR_BAD_ARGUMENT, std::string(who) + ": null para_Feature");
+            std::memcpy(hl.data() + w * dst.lam.per, states[w].para_Feature, (size_t)h->nfeat[w] * 8);
+        }
+    }
+    double *dlc = B.up(hl.data(), hl.size(), s);
+    if (!dlc) return fail(CERB_ERR_CUDA, "device allocation failed");
+    CUDA_TRY(cudaMemcpyAsync(dst.state.d, hst.data(), dst.state.bytes(n), cudaMemcpyHostToDevice, s));
+    CERB_LAUNCH(permute_lam_kernel, (int)(((size_t)n * F + 127) / 128), 128, 0, s, n, F, (const int *)h->n_features.d, (const int *)h->perm.d, (const double *)dlc, dst.lam.d);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(s));               // hst / hl are read by the asynchronous copies
+    return CERB_OK;
+}
+
 int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindowState *states, CerbPrior *priors, int32_t *sweeps) {
     if (!h || !flags || !priors) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: null argument");
     CERB_DEVICE(h);
-    const int n = h->n, F = h->F;
+    const int n = h->n;
     if (n < 1) return fail(CERB_ERR_BAD_ARGUMENT, "no resident batch");
     for (int w = 0; w < n; w++) {
         if (flags[w] != 0 && flags[w] != 1) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: flag must be 0 (MARGIN_OLD) or 1 (MARGIN_SECOND_NEW)");
@@ -883,27 +938,22 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
     const int nmax = MARG_N_STRUCT;            // what a window can keep (the kernel skips a window that claims more); the prior arrays keep the stride CERB_MAX_PRIOR_DIM
     for (int w = 0; w < n; w++) if (flags[w] == 0) mmax = std::max(mmax, 19 + h->n0[w]);
     const int posmax = mmax + CERB_MAX_PRIOR_DIM;
-    // states to linearise at: the caller's (after double2vector + vector2double), or the resident ones
-    std::vector<double> hst((size_t)n * ST_STRIDE, 0.0);
-    const double *d_st, *d_lm;
+    // states to linearise at: the caller's (after double2vector + vector2double), or the resident ones; hst is their host image
+    std::vector<double> hst;
+    States lin = resident_states(h);
     if (states) {
-        std::vector<double> hl((size_t)n * F, 0.0);
-        for (int w = 0; w < n; w++) {
-            std::memcpy(hst.data() + (size_t)w * ST_STRIDE, &states[w], ST_SIZE * sizeof(double));
-            if (h->nfeat[w]) { if (!states[w].para_Feature) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: null para_Feature"); std::memcpy(hl.data() + (size_t)w * F, states[w].para_Feature, (size_t)h->nfeat[w] * 8); }
-        }
-        double *ds = B.up(hst.data(), hst.size(), s), *dlc = B.up(hl.data(), hl.size(), s), *dl = B.up(nullptr, (size_t)n * F, s);
-        if (!ds || !dlc || !dl) return fail(CERB_ERR_CUDA, "device allocation failed");
-        CERB_LAUNCH(permute_lam_kernel, (int)(((size_t)n * F + 127) / 128), 128, 0, s, n, F, (const int *)h->d_nfeat, (const int *)h->d_perm, (const double *)dlc, dl);
-        CUDA_TRY(cudaStreamSynchronize(s));               // hl / hst are read by the asynchronous copies
-        d_st = ds; d_lm = dl;
+        lin.state.d = B.up(nullptr, n * lin.state.per, s); lin.lam.d = B.up(nullptr, n * lin.lam.per, s);
+        if (!lin.state.d || !lin.lam.d) return fail(CERB_ERR_CUDA, "device allocation failed");
+        int rc = states_to_device(h, B, states, "cerb_batch_marginalize", lin, hst); if (rc) return rc;
     } else {
-        d_st = h->solved ? h->d_state : h->d_state0; d_lm = h->solved ? h->d_lam : h->d_lam0;
-        CUDA_TRY(cudaMemcpyAsync(hst.data(), d_st, hst.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+        hst.resize(n * lin.state.per);
+        CUDA_TRY(cudaMemcpyAsync(hst.data(), lin.state.d, lin.state.bytes(n), cudaMemcpyDeviceToHost, s));
     }
     std::vector<int> hflags(flags, flags + n);
     int *dflags = B.upi(hflags.data(), n, s), *ddims = B.upi(nullptr, (size_t)n * 4, s), *dblocks = B.upi(nullptr, (size_t)n * 64, s), *dsw = B.upi(nullptr, (size_t)n * 2, s);
-    double *dJ = B.up(nullptr, (size_t)n * PRIOR_LD * PRIOR_LD, s), *dr = B.up(nullptr, (size_t)n * PRIOR_LD, s);
+    // the new priors, laid out as the resident one: they come back through its pinned mirrors
+    const size_t jper = h->prior_J.per, rper = h->prior_r.per;
+    double *dJ = B.up(nullptr, n * jper, s), *dr = B.up(nullptr, n * rper, s);
     // A / b of a sub-batch and the per-CTA workspace of the eigen-solver: bounded device memory whatever the batch size
     const size_t a_bytes = (size_t)posmax * posmax * 8, budget = (size_t)3 << 30;
     const int per = (int)std::max<size_t>(1, std::min<size_t>(n, budget / a_bytes));
@@ -918,32 +968,28 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
     CUDA_TRY(cudaFuncSetAttribute(marg_assemble_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_bytes));
     for (int w0 = 0; w0 < n; w0 += per) {
         const int cn = std::min(per, n - w0);
-        // sqrt_info of the IMU-leg factors and the Gram matrix of the old prior (a solve leaves them behind; a bare upload does not)
-        const int nfac = cn * 10;
-        CERB_LAUNCH(imu_leg_prepare_kernel, (nfac + 1) / 2, 64, 0, s, nfac, (const double *)(h->d_pre + (size_t)w0 * 10 * PRE_STRIDE), h->d_sinfo + (size_t)w0 * 10 * 961);
-        CERB_LAUNCH(prior_prepare_kernel, cn, 256, (size_t)PRIOR_TROWS * PRIOR_TLD * sizeof(double), s, (const double *)(h->d_pJ + (size_t)w0 * PRIOR_LD * PRIOR_LD), (const int *)(h->d_pmeta + (size_t)w0 * PRIOR_META_STRIDE), h->d_pHp + (size_t)w0 * PRIOR_LD * PRIOR_LD);
+        enqueue_prepare(h, w0, cn, s);         // a solve leaves sqrt_info and the prior's Gram matrix behind; a bare upload does not
         SolveParams P = make_params(h, w0, cn, 0, nullptr, -1);
         MargParams M;
-        M.flags = dflags + w0; M.state = d_st + (size_t)w0 * ST_STRIDE; M.lam = d_lm + (size_t)w0 * F; M.A = dA; M.b = db; M.posmax = posmax;
+        M.flags = dflags + w0; M.state = lin.state.at(w0); M.lam = lin.lam.at(w0); M.A = dA; M.b = db; M.posmax = posmax;
         M.dims = ddims + (size_t)w0 * 4; M.blocks = dblocks + (size_t)w0 * 64;
         CERB_LAUNCH(marg_assemble_kernel, std::min(cn, h->grid), SOLVE_THREADS, h->smem_bytes, s, P, M);
         CERB_LAUNCH(marg_schur_kernel, std::min(cn, sgrid), marg_threads(mmax, nmax, lim), marg_smem_bytes(mmax, nmax, lim), s, cn, mmax, nmax, (const int *)(ddims + (size_t)w0 * 4), (const double *)dA, (long)posmax * posmax,
-                    (const double *)db, (long)posmax, 1e-8, dws, dJ + (size_t)w0 * PRIOR_LD * PRIOR_LD, (long)PRIOR_LD * PRIOR_LD, dr + (size_t)w0 * PRIOR_LD, (long)PRIOR_LD, dsw + (size_t)w0 * 2, (int)lim);
+                    (const double *)db, (long)posmax, 1e-8, dws, dJ + w0 * jper, (long)jper, dr + w0 * rper, (long)rper, dsw + (size_t)w0 * 2, (int)lim);
         CUDA_TRY(cudaGetLastError());
     }
     std::vector<int> hdims((size_t)n * 4), hblocks((size_t)n * 64), hsw((size_t)n * 2);
-    double *hJ = h->h_pJ, *hr = h->h_pr;       // the pinned staging of the prior upload is idle here: D2H at PCIe rate instead of through pageable memory
     CUDA_TRY(cudaMemcpyAsync(hdims.data(), ddims, hdims.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(hblocks.data(), dblocks, hblocks.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(hsw.data(), dsw, hsw.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hJ, dJ, (size_t)n * PRIOR_LD * PRIOR_LD * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hr, dr, (size_t)n * PRIOR_LD * sizeof(double), cudaMemcpyDeviceToHost, s));
+    // the pinned staging of the prior upload is idle here: D2H at PCIe rate instead of through pageable memory
+    CUDA_TRY(cudaMemcpyAsync(h->prior_J.h, dJ, h->prior_J.bytes(n), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(h->prior_r.h, dr, h->prior_r.bytes(n), cudaMemcpyDeviceToHost, s));
     // a prior that is carried over unchanged comes back from the device copy of the old one
-    std::vector<int> hmeta((size_t)n * PRIOR_META_STRIDE); std::vector<double> hx0((size_t)n * 16 * 9);
-    CUDA_TRY(cudaMemcpyAsync(hmeta.data(), h->d_pmeta, hmeta.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hx0.data(), h->d_px0, hx0.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    std::vector<int> hmeta(n * h->prior_meta.per); std::vector<double> hx0(n * h->prior_x0.per);
+    CUDA_TRY(cudaMemcpyAsync(hmeta.data(), h->prior_meta.d, h->prior_meta.bytes(n), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(hx0.data(), h->prior_x0.d, h->prior_x0.bytes(n), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
-    std::vector<double> oldJ, oldr;
     std::vector<StageJob> out_jobs; out_jobs.reserve(n);
     for (int w = 0; w < n; w++) if (hdims[4 * w + 2] == 1 && (hdims[4 * w] > mmax || hdims[4 * w + 1] > nmax)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: a window exceeds the structural size of the kept / dropped blocks");
     for (int w = 0; w < n; w++) {
@@ -954,22 +1000,15 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
         pr.valid = 0; pr.n = 0; pr.num_blocks = 0;
         if (status == 0) continue;
         if (status == 2) {                       // MARGIN_SECOND_NEW without para_Pose[WINDOW_SIZE - 1] in the old prior: unchanged (estimator.cpp:1380-1381)
-            const int *meta = hmeta.data() + (size_t)w * PRIOR_META_STRIDE;
-            if (!meta[0]) continue;
-            pr.valid = 1; pr.n = meta[1]; pr.num_blocks = meta[2];
-            for (int b = 0; b < pr.num_blocks; b++) {
-                pr.block_kind[b] = meta[4 + 3 * b]; pr.block_index[b] = meta[5 + 3 * b]; pr.block_col[b] = meta[6 + 3 * b];
-                for (int k = 0; k < 9; k++) pr.block_x0[b][k] = hx0[(size_t)w * 144 + 9 * b + k];
-            }
-            oldJ.resize((size_t)pr.n * pr.n); oldr.resize(pr.n);
-            CUDA_TRY(cudaMemcpy(oldJ.data(), h->d_pJ + (size_t)w * PRIOR_LD * PRIOR_LD, oldJ.size() * 8, cudaMemcpyDeviceToHost));
-            CUDA_TRY(cudaMemcpy(oldr.data(), h->d_pr + (size_t)w * PRIOR_LD, oldr.size() * 8, cudaMemcpyDeviceToHost));
-            std::memcpy(Jout, oldJ.data(), oldJ.size() * 8); std::memcpy(rout, oldr.data(), oldr.size() * 8);
+            decode_prior(hmeta.data() + w * h->prior_meta.per, hx0.data() + w * h->prior_x0.per, pr);
+            if (!pr.valid) continue;
+            CUDA_TRY(cudaMemcpyAsync(Jout, h->prior_J.at(w), (size_t)pr.n * pr.n * 8, cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(cudaMemcpyAsync(rout, h->prior_r.at(w), (size_t)pr.n * 8, cudaMemcpyDeviceToHost, s));
             continue;
         }
         const int nn = hdims[4 * w + 1], nb = hdims[4 * w + 3];
         pr.valid = 1; pr.n = nn; pr.num_blocks = nb;
-        const double *st = hst.data() + (size_t)w * ST_STRIDE;
+        const double *st = hst.data() + w * h->state.per;
         for (int b = 0; b < nb; b++) {
             const int *q = hblocks.data() + (size_t)w * 64 + 4 * b;
             pr.block_kind[b] = q[0]; pr.block_index[b] = q[1]; pr.block_col[b] = q[2];
@@ -977,9 +1016,10 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
             const double *x = st + prior_block_state_offset(q[0], q[3]);          // keep_block_data: the state the factors were linearised at
             for (int k = 0; k < 9; k++) pr.block_x0[b][k] = k < size ? x[k] : 0.0;
         }
-        out_jobs.push_back({Jout, hJ + (size_t)w * PRIOR_LD * PRIOR_LD, (size_t)nn * nn * 8});       // 59 KB per window: copied by a few threads below
-        std::memcpy(rout, hr + (size_t)w * PRIOR_LD, (size_t)nn * 8);
+        out_jobs.push_back({Jout, h->prior_J.h_at(w), (size_t)nn * nn * 8});       // 59 KB per window: copied by a few threads below
+        std::memcpy(rout, h->prior_r.h_at(w), (size_t)nn * 8);
     }
+    CUDA_TRY(cudaStreamSynchronize(s));          // the carried-over priors
     run_stage_jobs(out_jobs);
     return CERB_OK;
 }
@@ -988,45 +1028,9 @@ int cerb_batch_update_states(CerbHandle *h, int32_t n, const CerbWindowState *st
     if (!h || !states) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
     CERB_DEVICE(h);
     if (h->n < 1 || n != h->n) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_update_states: n must be the size of the resident batch");
-    const int F = h->F;
-    cudaStream_t s = h->stream; DevBuf B(h);
-    std::vector<double> hst((size_t)n * ST_STRIDE, 0.0), hl((size_t)n * F, 0.0);
-    for (int w = 0; w < n; w++) {
-        std::memcpy(hst.data() + (size_t)w * ST_STRIDE, &states[w], ST_SIZE * sizeof(double));
-        if (h->nfeat[w]) { if (!states[w].para_Feature) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_update_states: null para_Feature"); std::memcpy(hl.data() + (size_t)w * F, states[w].para_Feature, (size_t)h->nfeat[w] * 8); }
-    }
-    double *ds = B.up(hst.data(), hst.size(), s), *dlc = B.up(hl.data(), hl.size(), s);
-    if (!ds || !dlc) return fail(CERB_ERR_CUDA, "device allocation failed");
-    CUDA_TRY(cudaMemcpyAsync(h->d_state0, ds, hst.size() * sizeof(double), cudaMemcpyDeviceToDevice, s));
-    CERB_LAUNCH(permute_lam_kernel, (int)(((size_t)n * F + 127) / 128), 128, 0, s, n, F, (const int *)h->d_nfeat, (const int *)h->d_perm, (const double *)dlc, h->d_lam0);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaStreamSynchronize(s));               // hst / hl are read by the asynchronous copies
+    DevBuf B(h); std::vector<double> hst;
+    int rc = states_to_device(h, B, states, "cerb_batch_update_states", States{h->state0, h->lam0}, hst); if (rc) return rc;
     h->solved = false;                                 // the per-feature passes and a resident solve start from these states
-    return CERB_OK;
-}
-
-int cerb_batch_shift_depth(CerbHandle *h, double init_depth, int32_t *new_start_frame, double *depth, int32_t *keep) {
-    if (!h || !new_start_frame || !depth || !keep) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
-    CERB_DEVICE(h);
-    if (h->n < 1) return fail(CERB_ERR_BAD_ARGUMENT, "no resident batch");
-    const int n = h->n, F = h->F;
-    const size_t N = (size_t)n * F;
-    cudaStream_t s = h->stream; DevBuf B(h);
-    double *d_out = B.up(nullptr, 3 * N, s), *d_perm_out = B.up(nullptr, 3 * N, s);
-    if (!d_out || !d_perm_out) return fail(CERB_ERR_CUDA, "device allocation failed");
-    const double *d_st = h->solved ? h->d_state : h->d_state0, *d_lm = h->solved ? h->d_lam : h->d_lam0;
-    CERB_LAUNCH(shift_depth_kernel, (int)((N + 127) / 128), 128, 0, s, n, F, h->O, (const int *)h->d_nfeat, (const int *)h->d_fstart, (const int *)h->d_fnobs, (const int *)h->d_foff,
-                (const double *)h->d_obs, d_st, d_lm, init_depth, d_out);
-    CERB_LAUNCH(unpermute_kernel, (int)((N + 127) / 128), 128, 0, s, n, F, 3, (const int *)h->d_nfeat, (const int *)h->d_perm, (const double *)d_out, d_perm_out);
-    CUDA_TRY(cudaGetLastError());
-    std::vector<double> tmp(3 * N);
-    CUDA_TRY(cudaMemcpyAsync(tmp.data(), d_perm_out, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
-    for (int w = 0; w < n; w++)
-        for (int f = 0; f < h->nfeat[w]; f++) {
-            const size_t q = (size_t)w * F + f;
-            new_start_frame[q] = (int32_t)tmp[q]; depth[q] = tmp[N + q]; keep[q] = (int32_t)tmp[2 * N + q];
-        }
     return CERB_OK;
 }
 

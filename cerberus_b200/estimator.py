@@ -537,18 +537,9 @@ class NativeReplay:
     for all robots.  Same inputs and outputs as ReplayDriver(DeviceOps(...)); tests/test_replay.py compares the two."""
 
     def __init__(self, backend, pcfg, n, max_features=160, estimate_extrinsic=1, estimate_td=0):
-        L = backend.lib
-        L.cerb_replay_create.argtypes = [C.c_void_p, C.POINTER(abi.PreintConfig), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
-        L.cerb_replay_destroy.argtypes = [C.c_void_p]; L.cerb_replay_destroy.restype = None
-        L.cerb_replay_set_extrinsics.argtypes = [C.c_void_p, C.c_int32, abi.c_dp, abi.c_dp]
-        L.cerb_replay_seed_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, abi.c_dp, abi.c_dp, abi.c_dp, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(abi.Image), C.c_double]
-        L.cerb_replay_step.argtypes = [C.c_void_p, C.POINTER(abi.Image), C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_double, C.POINTER(abi.SolveReport)]
-        L.cerb_replay_path.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), abi.c_dp, C.c_int32]
-        L.cerb_replay_feature_ids.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
-        L.cerb_replay_timing.argtypes = [C.c_void_p, abi.c_dp, abi.c_dp]
         self.be, self.n = backend, n
         self.r = C.c_void_p()
-        backend._check(L.cerb_replay_create(backend.h, C.byref(pcfg), n, max_features, estimate_extrinsic, estimate_td, C.byref(self.r)))
+        backend._check(backend.lib.cerb_replay_create(backend.h, C.byref(pcfg), n, max_features, estimate_extrinsic, estimate_td, C.byref(self.r)))
         self.reports = []
 
     def close(self):
@@ -620,7 +611,6 @@ class NativeReplay:
 
     def flag_history(self, w):
         n = C.c_int32(); out = np.zeros(4096, dtype=np.int32)
-        self.be.lib.cerb_replay_flags.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
         self.be._check(self.be.lib.cerb_replay_flags(self.r, w, C.byref(n), out.ctypes.data_as(C.POINTER(C.c_int32)), out.size))
         return out[:n.value]
 

@@ -67,6 +67,16 @@ class Backend:
         L.cerb_last_upload_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
         L.cerb_batch_marginalize.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(abi.WindowState), C.POINTER(abi.Prior), C.POINTER(C.c_int32)]
         L.cerb_double2vector.restype = None
+        L.cerb_replay_create.argtypes = [C.c_void_p, C.POINTER(abi.PreintConfig), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+        L.cerb_replay_destroy.argtypes = [C.c_void_p]
+        L.cerb_replay_destroy.restype = None
+        L.cerb_replay_set_extrinsics.argtypes = [C.c_void_p, C.c_int32, abi.c_dp, abi.c_dp]
+        L.cerb_replay_seed_frame.argtypes = [C.c_void_p, C.c_int32, C.c_int32, abi.c_dp, abi.c_dp, abi.c_dp, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(abi.Image), C.c_double]
+        L.cerb_replay_step.argtypes = [C.c_void_p, C.POINTER(abi.Image), C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.c_double, C.POINTER(abi.SolveReport)]
+        L.cerb_replay_path.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), abi.c_dp, C.c_int32]
+        L.cerb_replay_flags.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
+        L.cerb_replay_feature_ids.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
+        L.cerb_replay_timing.argtypes = [C.c_void_p, abi.c_dp, abi.c_dp]
         self.cfg = cfg or abi.default_config()
         self.h = C.c_void_p()
         self._check(L.cerb_create(C.byref(self.cfg), C.byref(self.h)))
