@@ -117,6 +117,14 @@ class PreintJob(C.Structure):
     ]
 
 
+class TrackPut(C.Structure):
+    _fields_ = [("window", C.c_int32), ("slot", C.c_int32), ("position", C.c_int32), ("reserved", C.c_int32), ("obs", Observation)]
+
+
+class TrackEdit(C.Structure):
+    _fields_ = [("window", C.c_int32), ("slot", C.c_int32), ("n_obs", C.c_int32), ("position", C.c_int32)]
+
+
 ABI_STRUCTS = [SolverConfig, IMULegPreint, Observation, Feature, Prior, WindowDesc, WindowState, SolveReport,
                IMULegSample, PreintConfig, PreintJob, IMUPreint]
 
@@ -126,6 +134,8 @@ preint_dtype = np.dtype(IMULegPreint)
 imu_preint_dtype = np.dtype(IMUPreint)
 sample_dtype = np.dtype(IMULegSample)
 report_dtype = np.dtype(SolveReport)
+track_put_dtype = np.dtype(TrackPut)
+track_edit_dtype = np.dtype(TrackEdit)
 
 
 def default_config():

@@ -9,6 +9,7 @@
 #include "feature_kernels.cuh"
 #include "marg_kernels.cuh"
 #include "pack_kernels.cuh"
+#include "resident_kernels.cuh"
 #include <string>
 #include <vector>
 #include <thread>
@@ -29,6 +30,16 @@ static int fail(int code, const std::string &msg) { g_err = msg; return code; }
         cudaError_t e_ = (expr);                                                                               \
         if (e_ != cudaSuccess) return fail(CERB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_)); \
     } while (0)
+// cudaMemcpyAsync between host and device, counted in the handle's traffic totals (cerb_traffic)
+#define COPY_TRY(h, dst, src, bytes, kind, s)                                                          \
+    do {                                                                                               \
+        (h)->traffic.count((kind), (bytes));                                                           \
+        CUDA_TRY(cudaMemcpyAsync((dst), (src), (bytes), (kind), (s)));                                 \
+    } while (0)
+struct Traffic {
+    int64_t h2d = 0, d2h = 0, ops = 0, staged = 0;
+    void count(cudaMemcpyKind kind, size_t bytes) { if (kind == cudaMemcpyDeviceToDevice) return; (kind == cudaMemcpyHostToDevice ? h2d : d2h) += (int64_t)bytes; ops++; }
+};
 
 // One array of the resident batch: `per` elements per window, window w at at(w); `h` is its pinned host mirror of the same shape, where it has one
 // (the staging of a caller's descriptors, the landing place of the results).
@@ -74,6 +85,13 @@ struct CerbHandle {
     size_t smem_bytes = 0;
     // scratch arena of the evaluator / feature / preintegration entry points: grows to the high-water mark, then no more cudaMalloc per call
     std::vector<std::pair<char *, size_t>> arena; size_t arena_chunk = 0, arena_used = 0;
+    Traffic traffic;                  // host <-> device copies issued since cerb_create
+    // resident sliding window (cerb_resident_*): robs / rpre / the prior of windows [0, res_n) are edited in place instead of uploaded
+    int res_n = 0; bool res_leg = true;
+    Resident<int> pre_slot;           // [B][CERB_WINDOW_SIZE] row of rpre that holds interval i -> i + 1
+    std::vector<int> res_extent;      // [B] observations of robs a pack has to read: up to the highest slot ever put
+    std::vector<char> res_prior_valid;
+    std::vector<unsigned char> res_mark;      // [B][O] scratch of the duplicate checks of put / edit (all zero between calls)
 };
 
 static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDeviceProp &prop);
@@ -184,7 +202,8 @@ static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDev
     CUDA_TRY(alloc(h, h->state, ST_STRIDE)); CUDA_TRY(alloc(h, h->state0, ST_STRIDE)); CUDA_TRY(alloc(h, h->lam, F)); CUDA_TRY(alloc(h, h->lam0, F)); CUDA_TRY(alloc(h, h->rep_d, 2));
     CUDA_TRY(dmalloc(h, &h->d_ws, (size_t)CerbHandle::LANES * h->grid * h->ws_stride)); CUDA_TRY(dmalloc(h, &h->d_dbg, 2 * (NR + F) + 8)); CUDA_TRY(dmalloc(h, &h->d_G, 4));
     CUDA_TRY(dmalloc(h, &h->d_probe_repi, 4)); CUDA_TRY(dmalloc(h, &h->d_probe_repd, 2)); CUDA_TRY(hmalloc(h, &h->h_dbg, 2 * (NR + F) + 8));
-    h->nfeat.assign(h->B, 0); h->n0.assign(h->B, 0);
+    CUDA_TRY(alloc(h, h->pre_slot, CERB_WINDOW_SIZE, true));
+    h->nfeat.assign(h->B, 0); h->n0.assign(h->B, 0); h->res_extent.assign(h->B, 0); h->res_prior_valid.assign(h->B, 0);
     CUDA_TRY(cudaMemcpy(h->d_G, cfg->g, 3 * sizeof(double), cudaMemcpyHostToDevice));
     return CERB_OK;
 }
@@ -285,18 +304,23 @@ static int validate_prior(const CerbPrior &pr) {
     return CERB_OK;
 }
 
-static int validate_window(const CerbHandle *h, const CerbWindowDesc &d, const CerbWindowState &st, int *n_anchor0) {
-    if (d.n_features < 0 || d.n_features > h->F) return fail(CERB_ERR_BAD_ARGUMENT, "window: n_features over capacity");
-    if (d.n_obs < 0 || d.n_obs > h->O) return fail(CERB_ERR_BAD_ARGUMENT, "window: n_obs over capacity");
-    if ((d.n_features && (!d.features || !d.obs || !st.para_Feature)) || (!d.preint && !d.imu_preint)) return fail(CERB_ERR_BAD_ARGUMENT, "window: null pointer");
+// the tracks of a feature list against an observation array of obs_bound records; *n_anchor0: tracks anchored at frame 0
+static int validate_tracks(const CerbWindowDesc &d, int obs_bound, int *n_anchor0) {
     int n0 = 0;
     for (int f = 0; f < d.n_features; f++) {
         const CerbFeature &ft = d.features[f];
-        if (ft.start_frame < 0 || ft.n_obs < 1 || ft.start_frame + ft.n_obs > CERB_NUM_FRAMES || ft.obs_offset < 0 || ft.obs_offset + ft.n_obs > d.n_obs)
+        if (ft.start_frame < 0 || ft.n_obs < 1 || ft.start_frame + ft.n_obs > CERB_NUM_FRAMES || ft.obs_offset < 0 || ft.obs_offset + ft.n_obs > obs_bound)
             return fail(CERB_ERR_BAD_ARGUMENT, "window: malformed feature track");
         n0 += ft.start_frame == 0;
     }
     if (n_anchor0) *n_anchor0 = n0;
+    return CERB_OK;
+}
+static int validate_window(const CerbHandle *h, const CerbWindowDesc &d, const CerbWindowState &st, int *n_anchor0) {
+    if (d.n_features < 0 || d.n_features > h->F) return fail(CERB_ERR_BAD_ARGUMENT, "window: n_features over capacity");
+    if (d.n_obs < 0 || d.n_obs > h->O) return fail(CERB_ERR_BAD_ARGUMENT, "window: n_obs over capacity");
+    if ((d.n_features && (!d.features || !d.obs || !st.para_Feature)) || (!d.preint && !d.imu_preint)) return fail(CERB_ERR_BAD_ARGUMENT, "window: null pointer");
+    const int rc = validate_tracks(d, d.n_obs, n_anchor0); if (rc) return rc;
     return validate_prior(d.prior);
 }
 
@@ -321,9 +345,25 @@ static void run_stage_jobs(const std::vector<StageJob> &jobs) {
     fan_out((int)jobs.size(), total >= (4u << 20), [&](int k) { std::memcpy(jobs[k].dst, jobs[k].src, jobs[k].bytes); return (int)CERB_OK; });
 }
 
+// stage what the plan stages, then issue its DMA operations on stream s
+static int run_plan(CerbHandle *h, const UploadPlan &pl, cudaStream_t s, double *t_stage_ms) {
+    const auto t0 = std::chrono::steady_clock::now();
+    run_stage_jobs(pl.stage);
+    if (t_stage_ms) *t_stage_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    for (const DmaOp &op : pl.dma) {
+        h->traffic.count(cudaMemcpyHostToDevice, op.width * op.height);
+        if (op.height == 1) CUDA_TRY(cudaMemcpyAsync(op.dst, op.src, op.width, cudaMemcpyHostToDevice, s));
+        else CUDA_TRY(cudaMemcpy2DAsync(op.dst, op.dpitch, op.src, op.spitch, op.width, op.height, cudaMemcpyHostToDevice, s));
+    }
+    const size_t staged = [&] { size_t t = 0; for (const auto &j : pl.stage) t += j.bytes; return t; }();
+    h->last_dma_ops += (int)pl.dma.size(); h->last_staged_bytes += staged; h->traffic.staged += (int64_t)staged;
+    return CERB_OK;
+}
+
 // validate windows [w0, w0 + cn), move their raw descriptors to the device on stream s (staging only what is not registered)
 static int upload_raw(CerbHandle *h, int w0, int cn, const CerbWindowDesc *descs, const CerbWindowState *states, cudaStream_t s, double *t_stage_ms) {
     for (int w = w0; w < w0 + cn; w++) { int rc = validate_window(h, descs[w], states[w], &h->n0[w]); if (rc) return rc; h->nfeat[w] = descs[w].n_features; }
+    h->res_n = 0;                      // robs / rpre / the prior are overwritten: the resident sliding window, if there was one, is gone
     UploadPlan pl;
     plan_rows(h, pl, w0, cn, h->rdesc, 0, 1, 0, [&](int w) { return (const void *)&descs[w]; }, [&](int) { return sizeof(CerbWindowDesc); });
     plan_rows(h, pl, w0, cn, h->rstate, 0, 1, 0, [&](int w) { return (const void *)&states[w]; }, [&](int) { return sizeof(CerbWindowState); });
@@ -348,15 +388,7 @@ static int upload_raw(CerbHandle *h, int w0, int cn, const CerbWindowDesc *descs
               [&](int w) { return (const void *)descs[w].prior.linearized_jacobians; }, [&](int w) { return descs[w].prior.valid ? (size_t)descs[w].prior.n * descs[w].prior.n * 8 : (size_t)0; });
     plan_rows(h, pl, w0, cn, h->prior_r, 0, 1, 0,
               [&](int w) { return (const void *)descs[w].prior.linearized_residuals; }, [&](int w) { return descs[w].prior.valid ? (size_t)descs[w].prior.n * 8 : (size_t)0; });
-    const auto t0 = std::chrono::steady_clock::now();
-    run_stage_jobs(pl.stage);
-    if (t_stage_ms) *t_stage_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    for (const DmaOp &op : pl.dma) {
-        if (op.height == 1) CUDA_TRY(cudaMemcpyAsync(op.dst, op.src, op.width, cudaMemcpyHostToDevice, s));
-        else CUDA_TRY(cudaMemcpy2DAsync(op.dst, op.dpitch, op.src, op.spitch, op.width, op.height, cudaMemcpyHostToDevice, s));
-    }
-    h->last_dma_ops += (int)pl.dma.size(); h->last_staged_bytes += [&] { size_t t = 0; for (const auto &j : pl.stage) t += j.bytes; return t; }();
-    return CERB_OK;
+    return run_plan(h, pl, s, t_stage_ms);
 }
 
 // device pack of windows [w0, w0 + cn) (after their raw descriptors have arrived) on stream s
@@ -367,6 +399,7 @@ static int enqueue_pack(CerbHandle *h, int w0, int cn, cudaStream_t s) {
     P.n_features = h->n_features.at(w0); P.feat_start = h->feat_start.at(w0); P.feat_nobs = h->feat_nobs.at(w0); P.feat_off = h->feat_off.at(w0); P.flags = h->flags.at(w0);
     P.obs_stereo = h->obs_stereo.at(w0); P.prior_meta = h->prior_meta.at(w0); P.perm = h->perm.at(w0);
     P.obs = h->obs.at(w0); P.pre = h->pre.at(w0); P.prior_x0 = h->prior_x0.at(w0); P.state0 = h->state0.at(w0); P.lam0 = h->lam0.at(w0);
+    if (h->res_n) P.pre_slot = h->pre_slot.at(w0);
     CERB_LAUNCH(pack_kernel, std::min(cn, 8 * h->sm_count), PACK_THREADS, 0, s, P);
     CUDA_TRY(cudaGetLastError());
     return CERB_OK;
@@ -463,9 +496,9 @@ static int download(CerbHandle *h, CerbWindowState *states, CerbSolveReport *rep
     U.olam = h->olam.d; U.orep = h->orep.d; U.ostate = h->ostate.d;
     CERB_LAUNCH(unpack_kernel, std::min(n, 8 * h->sm_count), PACK_THREADS, 0, s, U);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(h->ostate.h, h->ostate.d, h->ostate.bytes(n), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(h->olam.h, h->olam.d, h->olam.bytes(n), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(h->orep.h, h->orep.d, h->orep.bytes(n), cudaMemcpyDeviceToHost, s));
+    COPY_TRY(h, h->ostate.h, h->ostate.d, h->ostate.bytes(n), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, h->olam.h, h->olam.d, h->olam.bytes(n), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, h->orep.h, h->orep.d, h->orep.bytes(n), cudaMemcpyDeviceToHost, s);
     CUDA_TRY(cudaStreamSynchronize(s));
     int rc = collect_time(h); if (rc) return rc;
     int status = CERB_OK;
@@ -651,12 +684,12 @@ struct DevBuf {   // bump allocator over the handle's scratch arena (reset per e
     }
     double *up(const double *src, size_t n, cudaStream_t s) {
         double *d = (double *)raw(n * sizeof(double)); if (!d) return nullptr;
-        if (src) cudaMemcpyAsync(d, src, n * sizeof(double), cudaMemcpyHostToDevice, s);
+        if (src) { h->traffic.count(cudaMemcpyHostToDevice, n * sizeof(double)); cudaMemcpyAsync(d, src, n * sizeof(double), cudaMemcpyHostToDevice, s); }
         return d;
     }
     int *upi(const int *src, size_t n, cudaStream_t s) {
         int *d = (int *)raw(n * sizeof(int)); if (!d) return nullptr;
-        if (src) cudaMemcpyAsync(d, src, n * sizeof(int), cudaMemcpyHostToDevice, s);
+        if (src) { h->traffic.count(cudaMemcpyHostToDevice, n * sizeof(int)); cudaMemcpyAsync(d, src, n * sizeof(int), cudaMemcpyHostToDevice, s); }
         return d;
     }
 };
@@ -834,7 +867,7 @@ template <class Launch, class Store> static int feature_pass(CerbHandle *h, int 
     CERB_LAUNCH(unpermute_kernel, blocks, threads, 0, s, n, F, planes, (const int *)h->n_features.d, (const int *)h->perm.d, (const double *)d_out, d_perm_out);   // device slot -> caller's feature index
     CUDA_TRY(cudaGetLastError());
     std::vector<double> tmp(planes * N);
-    CUDA_TRY(cudaMemcpyAsync(tmp.data(), d_perm_out, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    COPY_TRY(h, tmp.data(), d_perm_out, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost, s);
     CUDA_TRY(cudaStreamSynchronize(s));
     for (int w = 0; w < n; w++)
         for (int f = 0; f < h->nfeat[w]; f++) store((size_t)w * F + f, tmp.data(), N);
@@ -917,21 +950,21 @@ static int states_to_device(CerbHandle *h, DevBuf &B, const CerbWindowState *sta
     }
     double *dlc = B.up(hl.data(), hl.size(), s);
     if (!dlc) return fail(CERB_ERR_CUDA, "device allocation failed");
-    CUDA_TRY(cudaMemcpyAsync(dst.state.d, hst.data(), dst.state.bytes(n), cudaMemcpyHostToDevice, s));
+    COPY_TRY(h, dst.state.d, hst.data(), dst.state.bytes(n), cudaMemcpyHostToDevice, s);
     CERB_LAUNCH(permute_lam_kernel, (int)(((size_t)n * F + 127) / 128), 128, 0, s, n, F, (const int *)h->n_features.d, (const int *)h->perm.d, (const double *)dlc, dst.lam.d);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaStreamSynchronize(s));               // hst / hl are read by the asynchronous copies
     return CERB_OK;
 }
 
-int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindowState *states, CerbPrior *priors, int32_t *sweeps) {
-    if (!h || !flags || !priors) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: null argument");
-    CERB_DEVICE(h);
+// cerb_batch_marginalize (priors: the new priors return to the host) and cerb_resident_marginalize (priors == NULL: they become the priors of
+// the resident windows on the device, valid [n] returns)
+static int marginalize_impl(CerbHandle *h, const int32_t *flags, const CerbWindowState *states, CerbPrior *priors, int32_t *sweeps, int32_t *valid) {
     const int n = h->n;
     if (n < 1) return fail(CERB_ERR_BAD_ARGUMENT, "no resident batch");
     for (int w = 0; w < n; w++) {
         if (flags[w] != 0 && flags[w] != 1) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: flag must be 0 (MARGIN_OLD) or 1 (MARGIN_SECOND_NEW)");
-        if (!priors[w].linearized_jacobians || !priors[w].linearized_residuals) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: priors[w] needs storage for linearized_jacobians / linearized_residuals");
+        if (priors && (!priors[w].linearized_jacobians || !priors[w].linearized_residuals)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: priors[w] needs storage for linearized_jacobians / linearized_residuals");
     }
     cudaStream_t s = h->stream; DevBuf B(h);
     int mmax = 19;
@@ -947,7 +980,7 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
         int rc = states_to_device(h, B, states, "cerb_batch_marginalize", lin, hst); if (rc) return rc;
     } else {
         hst.resize(n * lin.state.per);
-        CUDA_TRY(cudaMemcpyAsync(hst.data(), lin.state.d, lin.state.bytes(n), cudaMemcpyDeviceToHost, s));
+        COPY_TRY(h, hst.data(), lin.state.d, lin.state.bytes(n), cudaMemcpyDeviceToHost, s);
     }
     std::vector<int> hflags(flags, flags + n);
     int *dflags = B.upi(hflags.data(), n, s), *ddims = B.upi(nullptr, (size_t)n * 4, s), *dblocks = B.upi(nullptr, (size_t)n * 64, s), *dsw = B.upi(nullptr, (size_t)n * 2, s);
@@ -979,16 +1012,31 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
         CUDA_TRY(cudaGetLastError());
     }
     std::vector<int> hdims((size_t)n * 4), hblocks((size_t)n * 64), hsw((size_t)n * 2);
-    CUDA_TRY(cudaMemcpyAsync(hdims.data(), ddims, hdims.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hblocks.data(), dblocks, hblocks.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hsw.data(), dsw, hsw.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (!priors) {
+        // the old prior was an input of the kernels above: it is replaced only now, by a kernel behind them on the stream
+        COPY_TRY(h, hdims.data(), ddims, hdims.size() * sizeof(int), cudaMemcpyDeviceToHost, s);
+        CUDA_TRY(cudaStreamSynchronize(s));
+        for (int w = 0; w < n; w++) if (hdims[4 * w + 2] == 1 && (hdims[4 * w] > mmax || hdims[4 * w + 1] > nmax)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_resident_marginalize: a window exceeds the structural size of the kept / dropped blocks");
+        CERB_LAUNCH(prior_handover_kernel, std::min(n, 8 * h->sm_count), 256, 0, s, n, (const int *)ddims, (const int *)dblocks, (const double *)lin.state.d, (const double *)dJ, (long)jper,
+                    (const double *)dr, (long)rper, h->rdesc.d, h->prior_J.d, h->prior_r.d);
+        CUDA_TRY(cudaGetLastError());
+        for (int w = 0; w < n; w++) {
+            const int status = hdims[4 * w + 2];
+            if (status != 2) h->res_prior_valid[w] = status == 1;
+            valid[w] = h->res_prior_valid[w];
+        }
+        return CERB_OK;
+    }
+    COPY_TRY(h, hdims.data(), ddims, hdims.size() * sizeof(int), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, hblocks.data(), dblocks, hblocks.size() * sizeof(int), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, hsw.data(), dsw, hsw.size() * sizeof(int), cudaMemcpyDeviceToHost, s);
     // the pinned staging of the prior upload is idle here: D2H at PCIe rate instead of through pageable memory
-    CUDA_TRY(cudaMemcpyAsync(h->prior_J.h, dJ, h->prior_J.bytes(n), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(h->prior_r.h, dr, h->prior_r.bytes(n), cudaMemcpyDeviceToHost, s));
+    COPY_TRY(h, h->prior_J.h, dJ, h->prior_J.bytes(n), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, h->prior_r.h, dr, h->prior_r.bytes(n), cudaMemcpyDeviceToHost, s);
     // a prior that is carried over unchanged comes back from the device copy of the old one
     std::vector<int> hmeta(n * h->prior_meta.per); std::vector<double> hx0(n * h->prior_x0.per);
-    CUDA_TRY(cudaMemcpyAsync(hmeta.data(), h->prior_meta.d, h->prior_meta.bytes(n), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hx0.data(), h->prior_x0.d, h->prior_x0.bytes(n), cudaMemcpyDeviceToHost, s));
+    COPY_TRY(h, hmeta.data(), h->prior_meta.d, h->prior_meta.bytes(n), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, hx0.data(), h->prior_x0.d, h->prior_x0.bytes(n), cudaMemcpyDeviceToHost, s);
     CUDA_TRY(cudaStreamSynchronize(s));
     std::vector<StageJob> out_jobs; out_jobs.reserve(n);
     for (int w = 0; w < n; w++) if (hdims[4 * w + 2] == 1 && (hdims[4 * w] > mmax || hdims[4 * w + 1] > nmax)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: a window exceeds the structural size of the kept / dropped blocks");
@@ -1002,8 +1050,8 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
         if (status == 2) {                       // MARGIN_SECOND_NEW without para_Pose[WINDOW_SIZE - 1] in the old prior: unchanged (estimator.cpp:1380-1381)
             decode_prior(hmeta.data() + w * h->prior_meta.per, hx0.data() + w * h->prior_x0.per, pr);
             if (!pr.valid) continue;
-            CUDA_TRY(cudaMemcpyAsync(Jout, h->prior_J.at(w), (size_t)pr.n * pr.n * 8, cudaMemcpyDeviceToHost, s));
-            CUDA_TRY(cudaMemcpyAsync(rout, h->prior_r.at(w), (size_t)pr.n * 8, cudaMemcpyDeviceToHost, s));
+            COPY_TRY(h, Jout, h->prior_J.at(w), (size_t)pr.n * pr.n * 8, cudaMemcpyDeviceToHost, s);
+            COPY_TRY(h, rout, h->prior_r.at(w), (size_t)pr.n * 8, cudaMemcpyDeviceToHost, s);
             continue;
         }
         const int nn = hdims[4 * w + 1], nb = hdims[4 * w + 3];
@@ -1024,6 +1072,12 @@ int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindow
     return CERB_OK;
 }
 
+int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindowState *states, CerbPrior *priors, int32_t *sweeps) {
+    if (!h || !flags || !priors) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_batch_marginalize: null argument");
+    CERB_DEVICE(h);
+    return marginalize_impl(h, flags, states, priors, sweeps, nullptr);
+}
+
 int cerb_batch_update_states(CerbHandle *h, int32_t n, const CerbWindowState *states) {
     if (!h || !states) return fail(CERB_ERR_BAD_ARGUMENT, "null argument");
     CERB_DEVICE(h);
@@ -1035,11 +1089,13 @@ int cerb_batch_update_states(CerbHandle *h, int32_t n, const CerbWindowState *st
 }
 
 // ---- leg-contact preintegration ------------------------------------------------------------------------------------
-static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, CerbIMULegPreint *out, CerbIMUPreint *out_imu) {
-    if (!h || !cfg || n < 1 || !jobs || (!out && !out_imu)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_preintegrate: bad argument");
+// where (resident sliding window): [n][2] window, slot -- the results stay in rpre and only sum_dt [n] returns; else out / out_imu receive them
+static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, CerbIMULegPreint *out, CerbIMUPreint *out_imu,
+                             const int *where = nullptr, double *sum_dt = nullptr) {
+    if (!h || !cfg || n < 1 || !jobs || (!out && !out_imu && !where)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_preintegrate: bad argument");
     CERB_DEVICE(h);
     PreintParams P;
-    P.imu_only = out_imu ? 1 : 0;
+    P.imu_only = where ? (h->res_leg ? 0 : 1) : (out_imu ? 1 : 0);
     P.acc_n = cfg->acc_n; P.acc_n_z = cfg->acc_n_z; P.gyr_n = cfg->gyr_n; P.acc_w = cfg->acc_w; P.gyr_w = cfg->gyr_w; P.phi_n = cfg->phi_n; P.dphi_n = cfg->dphi_n;
     P.rho_c_n = cfg->rho_c_n; P.rho_nc_n = cfg->rho_nc_n; P.v_n_min_xy = cfg->v_n_min_xy; P.v_n_min_z = cfg->v_n_min_z; P.v_n_min = cfg->v_n_min; P.v_n_max = cfg->v_n_max;
     P.v_n_force_thres_ratio = cfg->v_n_force_thres_ratio; P.v_n_term1_steep = cfg->v_n_term1_steep; P.v_n_term2_var_rescale = cfg->v_n_term2_var_rescale;
@@ -1071,9 +1127,20 @@ static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t
     if (!dj || !ds || !dout || !dfull || !di) return fail(CERB_ERR_CUDA, "device allocation failed");
     CERB_LAUNCH(preintegrate_kernel, n, 128, 0, s, P, (int)n, (const double *)dj, (const int *)di, (const double *)ds, dout, dfull);
     CUDA_TRY(cudaGetLastError());
+    if (where) {
+        int *dwhere = B.upi(where, (size_t)n * 2, s); double *dsum = B.up(nullptr, n, s);
+        if (!dwhere || !dsum) return fail(CERB_ERR_CUDA, "device allocation failed");
+        CERB_LAUNCH(preint_store_kernel, n, 128, 0, s, (int)n, P.imu_only, (const int *)dwhere, (const double *)dout, (const double *)dfull, h->rpre.d, dsum);
+        CUDA_TRY(cudaGetLastError());
+        std::vector<double> hsum(n);
+        COPY_TRY(h, hsum.data(), dsum, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s);
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (sum_dt) std::memcpy(sum_dt, hsum.data(), (size_t)n * sizeof(double));
+        return CERB_OK;
+    }
     std::vector<double> ho((size_t)n * PRE_STRIDE), hf((size_t)n * 1922);
-    CUDA_TRY(cudaMemcpyAsync(ho.data(), dout, ho.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaMemcpyAsync(hf.data(), dfull, hf.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    COPY_TRY(h, ho.data(), dout, ho.size() * sizeof(double), cudaMemcpyDeviceToHost, s);
+    COPY_TRY(h, hf.data(), dfull, hf.size() * sizeof(double), cudaMemcpyDeviceToHost, s);
     CUDA_TRY(cudaStreamSynchronize(s));
     for (int j = 0; j < n; j++) {
         const double *o = ho.data() + (size_t)j * PRE_STRIDE, *f = hf.data() + (size_t)j * 1922;
@@ -1131,4 +1198,5 @@ void cerb_double2vector(const CerbWindowState *before, const CerbWindowState *af
 
 }  // extern "C"
 
+#include "resident_host.inl"
 #include "replay_host.inl"

@@ -23,6 +23,7 @@ struct PackParams {
     const CerbWindowDesc *rdesc; const CerbFeature *rfeat; const CerbObservation *robs; const double *rpre; const CerbWindowState *rstate; const double *rlam;
     int *n_features, *feat_start, *feat_nobs, *feat_off, *flags, *obs_stereo, *prior_meta, *perm;
     double *obs, *pre, *prior_x0, *state0, *lam0;
+    const int *pre_slot = nullptr;       // [n][CERB_WINDOW_SIZE] row of rpre that holds interval i -> i + 1 (resident sliding window); null: row i
 };
 
 CERB_HD double pack_pre_leg(const double *raw, int k) {
@@ -117,7 +118,7 @@ CERB_GLOBAL void __launch_bounds__(PACK_THREADS) pack_kernel(CERB_GRID_CONSTANT 
         // ---- preintegration records ----------------------------------------------------------------------------------
         for (int e = tid; e < CERB_WINDOW_SIZE * PRE_STRIDE; e += PACK_THREADS) {
             const int i = e / PRE_STRIDE, k = e % PRE_STRIDE;
-            const double *raw = P.rpre + ((size_t)w * CERB_WINDOW_SIZE + i) * RAW_PRE_STRIDE;
+            const double *raw = P.rpre + ((size_t)w * CERB_WINDOW_SIZE + (P.pre_slot ? P.pre_slot[w * CERB_WINDOW_SIZE + i] : i)) * RAW_PRE_STRIDE;
             P.pre[((size_t)w * CERB_WINDOW_SIZE + i) * PRE_STRIDE + k] = leg ? pack_pre_leg(raw, k) : pack_pre_imu(raw, k);
         }
         // ---- prior block list -----------------------------------------------------------------------------------------

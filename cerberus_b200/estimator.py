@@ -536,10 +536,14 @@ class NativeReplay:
     """The same lock-step replay with the host side in C++ inside the library (csrc/replay_host.inl, cerb_replay_*): one call per camera frame
     for all robots.  Same inputs and outputs as ReplayDriver(DeviceOps(...)); tests/test_replay.py compares the two."""
 
-    def __init__(self, backend, pcfg, n, max_features=160, estimate_extrinsic=1, estimate_td=0):
+    def __init__(self, backend, pcfg, n, max_features=160, estimate_extrinsic=1, estimate_td=0, resident=False):
+        """resident=True: every robot's window stays on the device across frames (cerb_resident_*) and a step sends the frame's edits
+        instead of three full uploads; same trajectories bit for bit."""
         self.be, self.n = backend, n
         self.r = C.c_void_p()
         backend._check(backend.lib.cerb_replay_create(backend.h, C.byref(pcfg), n, max_features, estimate_extrinsic, estimate_td, C.byref(self.r)))
+        if resident:
+            backend._check(backend.lib.cerb_replay_set_resident(self.r, 1))
         self.reports = []
 
     def close(self):
@@ -618,6 +622,27 @@ class NativeReplay:
         dev = np.zeros(6); host = C.c_double()
         self.be._check(self.be.lib.cerb_replay_timing(self.r, dev.ctypes.data_as(abi.c_dp), C.cast(C.byref(host), abi.c_dp)))
         return dict(zip(("preintegrate", "triangulate", "solve", "marginalize", "outliers", "shift"), dev.tolist()), host=host.value)
+
+    def traffic(self):
+        """What the steps so far asked the library to move: bytes host -> device and device -> host, copy operations, and the bytes of it
+        that went through a staging memcpy on the host."""
+        v = [C.c_int64() for _ in range(4)]
+        self.be._check(self.be.lib.cerb_replay_traffic(self.r, *[C.byref(x) for x in v]))
+        return dict(zip(("h2d_bytes", "d2h_bytes", "dma_ops", "staged_bytes"), [x.value for x in v]))
+
+    def window(self, w):
+        """cerb_replay_window: (features, ids, obs, preint [10], preint_current [10], pre_slots [10], Prior, prior_J [n, n], prior_r [n]) of
+        robot w as the replay would upload it for a per-feature step; in resident mode obs / preint are empty and prior carries valid only."""
+        d = abi.WindowDesc(); ids = np.zeros(4096, dtype=np.int32); cur = np.zeros(WINDOW_SIZE, dtype=np.int32); slots = np.zeros(WINDOW_SIZE, dtype=np.int32)
+        i32p = C.POINTER(C.c_int32)
+        self.be._check(self.be.lib.cerb_replay_window(self.r, w, C.byref(d), ids.ctypes.data_as(i32p), ids.size, cur.ctypes.data_as(i32p), slots.ctypes.data_as(i32p)))
+        take = lambda ptr, n, dt: np.ctypeslib.as_array(ptr, shape=(n,)).view(dt).reshape(n).copy() if n else np.zeros(0, dtype=dt)
+        feats = take(d.features, d.n_features, abi.feature_dtype); obs = take(d.obs, d.n_obs, abi.obs_dtype)
+        pre = take(d.preint, WINDOW_SIZE, abi.preint_dtype) if d.n_obs else np.zeros(0, dtype=abi.preint_dtype)
+        n = d.prior.n if (d.prior.valid and d.prior.linearized_jacobians) else 0
+        J = np.ctypeslib.as_array(d.prior.linearized_jacobians, shape=(n * n,)).reshape(n, n).T.copy() if n else np.zeros((0, 0))
+        r = np.ctypeslib.as_array(d.prior.linearized_residuals, shape=(n,)).copy() if n else np.zeros(0)
+        return feats, ids[:d.n_features], obs, pre, cur, slots, d.prior, J, r
 
 
 def write_csv(path, est, pcfg):

@@ -77,6 +77,19 @@ class Backend:
         L.cerb_replay_flags.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
         L.cerb_replay_feature_ids.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
         L.cerb_replay_timing.argtypes = [C.c_void_p, abi.c_dp, abi.c_dp]
+        i32p, i64p = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
+        L.cerb_replay_set_resident.argtypes = [C.c_void_p, C.c_int32]
+        L.cerb_replay_traffic.argtypes = [C.c_void_p, i64p, i64p, i64p, i64p]
+        L.cerb_replay_window.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.WindowDesc), i32p, C.c_int32, i32p, i32p]
+        L.cerb_resident_start.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+        L.cerb_resident_put_observations.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.TrackPut)]
+        L.cerb_resident_edit_tracks.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.TrackEdit)]
+        L.cerb_resident_preintegrate.argtypes = [C.c_void_p, C.POINTER(abi.PreintConfig), C.c_int32, C.POINTER(abi.PreintJob), i32p, i32p, abi.c_dp]
+        L.cerb_resident_upload.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.WindowDesc), C.POINTER(abi.WindowState), i32p]
+        L.cerb_resident_marginalize.argtypes = [C.c_void_p, i32p, C.POINTER(abi.WindowState), i32p]
+        L.cerb_resident_set_prior.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Prior)]
+        L.cerb_resident_read_window.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Observation), C.POINTER(abi.IMULegPreint), C.POINTER(abi.IMUPreint), C.POINTER(abi.Prior)]
+        L.cerb_traffic.argtypes = [C.c_void_p, i64p, i64p, i64p]
         self.cfg = cfg or abi.default_config()
         self.h = C.c_void_p()
         self._check(L.cerb_create(C.byref(self.cfg), C.byref(self.h)))
@@ -225,6 +238,58 @@ class Backend:
         depth = np.full((n, self.cfg.max_features), np.nan)
         self._check(self.lib.cerb_batch_triangulate(self.h, init_depth, _p(depth)))
         return depth
+
+    # ---- resident sliding window: tracks, preintegrations and the prior stay on the device, the host sends edits ----------
+    def resident_start(self, n, use_leg=True):
+        self._check(self.lib.cerb_resident_start(self.h, n, 1 if use_leg else 0))
+
+    def resident_put(self, puts):
+        """puts: array of abi.track_put_dtype (window, slot, position, obs)"""
+        puts = np.ascontiguousarray(puts, dtype=abi.track_put_dtype)
+        self._check(self.lib.cerb_resident_put_observations(self.h, len(puts), puts.ctypes.data_as(C.POINTER(abi.TrackPut))))
+
+    def resident_edit(self, edits):
+        """edits: array of abi.track_edit_dtype (window, slot, n_obs, position): erase observation `position` of each listed track"""
+        edits = np.ascontiguousarray(edits, dtype=abi.track_edit_dtype)
+        self._check(self.lib.cerb_resident_edit_tracks(self.h, len(edits), edits.ctypes.data_as(C.POINTER(abi.TrackEdit))))
+
+    def resident_preintegrate(self, pcfg, jobs, n, windows, slots):
+        """job j's result into preintegration slot slots[j] of window windows[j]; returns sum_dt [n]"""
+        windows = np.ascontiguousarray(windows, dtype=np.int32); slots = np.ascontiguousarray(slots, dtype=np.int32)
+        sum_dt = np.zeros(n)
+        self._check(self.lib.cerb_resident_preintegrate(self.h, C.byref(pcfg), n, jobs, windows.ctypes.data_as(C.POINTER(C.c_int32)), slots.ctypes.data_as(C.POINTER(C.c_int32)), _p(sum_dt)))
+        return sum_dt
+
+    def resident_upload(self, batch, pre_slots=None):
+        """feature lists (obs_offset = slot * NUM_FRAMES), open flags and states of batch against the resident data; pre_slots [n, 10]"""
+        ps = np.ascontiguousarray(np.tile(np.arange(abi.WINDOW_SIZE), (batch.n, 1)) if pre_slots is None else pre_slots, dtype=np.int32)
+        self._check(self.lib.cerb_resident_upload(self.h, batch.n, batch.descs, batch.states, ps.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def resident_marginalize(self, flags, states):
+        flags = np.ascontiguousarray(flags, dtype=np.int32); valid = np.zeros(len(flags), dtype=np.int32)
+        self._check(self.lib.cerb_resident_marginalize(self.h, flags.ctypes.data_as(C.POINTER(C.c_int32)), states, valid.ctypes.data_as(C.POINTER(C.c_int32))))
+        return valid
+
+    def resident_set_prior(self, w, prior):
+        self._check(self.lib.cerb_resident_set_prior(self.h, w, C.byref(prior)))
+
+    def resident_read_window(self, w, use_leg=True):
+        """One window's store: (obs [max_obs] slot by slot, preintegration records [10] by slot, Prior, prior_J [n, n], prior_r [n])."""
+        obs = np.zeros(self.cfg.max_obs, dtype=abi.obs_dtype)
+        pre = np.zeros(abi.WINDOW_SIZE, dtype=abi.preint_dtype if use_leg else abi.imu_preint_dtype)
+        J, r = np.zeros(abi.MAX_PRIOR_DIM * abi.MAX_PRIOR_DIM), np.zeros(abi.MAX_PRIOR_DIM)
+        pr = abi.Prior(); pr.linearized_jacobians = _p(J); pr.linearized_residuals = _p(r)
+        self._check(self.lib.cerb_resident_read_window(self.h, w, obs.ctypes.data_as(C.POINTER(abi.Observation)),
+                                                       pre.ctypes.data_as(C.POINTER(abi.IMULegPreint)) if use_leg else None,
+                                                       None if use_leg else pre.ctypes.data_as(C.POINTER(abi.IMUPreint)), C.byref(pr)))
+        n = pr.n if pr.valid else 0
+        return obs, pre, pr, J[:n * n].reshape(n, n).T.copy(), r[:n].copy()
+
+    def traffic(self):
+        """bytes host -> device, device -> host and copy operations issued by this handle so far"""
+        a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
+        self._check(self.lib.cerb_traffic(self.h, C.byref(a), C.byref(b), C.byref(c)))
+        return dict(h2d_bytes=a.value, d2h_bytes=b.value, dma_ops=c.value)
 
     # ---- synth backend protocol -----------------------------------------------------------------------------
     def preintegrate(self, pcfg, jobs, n):

@@ -401,6 +401,61 @@ int cerb_marginalize_schur(CerbHandle *h, int32_t n_windows, int32_t m, int32_t 
  * Kept-block order: poses ascending, speed bias, leg bias, ex0, ex1, td (the reference's order is that of an unordered_map keyed by pointer). */
 int cerb_batch_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindowState *states, CerbPrior *priors, int32_t *sweeps);
 
+/* ---- resident sliding window: the tracks, the preintegrations and the prior of n windows stay in HBM across frames; the host sends edits ------
+ * A second way to feed the resident batch, next to cerb_batch_upload.  Between two frames of one robot almost nothing of a window changes
+ * (Estimator::processImage -> slideWindow, estimator.cpp:655-846, 1460-1677): one frame of observations arrives, one interval is
+ * preintegrated, the prior is replaced by the one the marginalization has just computed.  The host keeps the bookkeeping (feature ids,
+ * start_frame, list order, depths, the keyframe test, double2vector); the device keeps the data:
+ *   track store     the raw observation array of a window used as max_obs / CERB_NUM_FRAMES fixed slots of CERB_NUM_FRAMES observations;
+ *                   a track lives left-aligned in one slot and CerbFeature.obs_offset = slot * CERB_NUM_FRAMES addresses it.  Which slots
+ *                   are free is the caller's knowledge.
+ *   preintegrations CERB_WINDOW_SIZE slots per window; the resident upload names the slot of every interval i -> i + 1, so a slide is a
+ *                   rotation of that table, not a copy
+ *   prior           written by cerb_resident_marginalize (or cerb_resident_set_prior) and read by the next cerb_resident_upload
+ * Every call validates its arguments before anything is launched (CERB_ERR_BAD_ARGUMENT leaves the store as it was).  cerb_batch_upload and
+ * cerb_solve_batch overwrite the store: they end the resident mode of the handle. */
+typedef struct CerbTrackPut {          /* FeaturePerId::feature_per_frame.push_back (feature_manager.cpp:93-113) */
+    int32_t window, slot, position, reserved;      /* observation `position` (0 = the anchor frame's) of the track in `slot` */
+    CerbObservation obs;
+} CerbTrackPut;
+typedef struct CerbTrackEdit {         /* feature_per_frame.erase(begin() + position): position 0 for removeBackShiftDepth / removeBack
+                                          (feature_manager.cpp:450-506), WINDOW_SIZE - 1 - start_frame for removeFront (:508-529) */
+    int32_t window, slot, n_obs, position;         /* n_obs: observations the track holds before the edit */
+} CerbTrackEdit;
+/* Start n resident windows with empty stores, identity slot tables and no prior.  use_leg: 1 = CerbIMULegPreint records (USE_LEG == 1),
+ * 0 = CerbIMUPreint records. */
+int cerb_resident_start(CerbHandle *h, int32_t n, int32_t use_leg);
+/* Scatter observations into the track stores / apply one erase per listed track (a track may be listed once per call). */
+int cerb_resident_put_observations(CerbHandle *h, int32_t count, const CerbTrackPut *puts);
+int cerb_resident_edit_tracks(CerbHandle *h, int32_t count, const CerbTrackEdit *edits);
+/* cerb_preintegrate_batch / cerb_preintegrate_imu_batch (by the use_leg of cerb_resident_start) with the result of job j left in
+ * preintegration slot slots[j] of window windows[j], in the layout an upload of the record would have produced; only sum_dt (optional,
+ * [n]) returns to the host.  slideWindowNew's merge of two intervals (estimator.cpp:1576-1616) is one job over both sample buffers. */
+int cerb_resident_preintegrate(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, const int32_t *windows,
+                               const int32_t *slots, double *sum_dt);
+/* cerb_batch_upload against the resident data: of descs[w] only n_features, features (obs_offset = slot * CERB_NUM_FRAMES), extrinsic_open
+ * and td_open are read; states as in cerb_batch_upload; pre_slots [n][CERB_WINDOW_SIZE]: slot of interval i -> i + 1, a permutation of
+ * 0 .. CERB_WINDOW_SIZE - 1 per window.  n must be the n of cerb_resident_start.  Afterwards the resident batch is used as after
+ * cerb_batch_upload (cerb_batch_solve_resident, cerb_batch_download, the per-feature steps, cerb_batch_update_states). */
+int cerb_resident_upload(CerbHandle *h, int32_t n, const CerbWindowDesc *descs, const CerbWindowState *states, const int32_t *pre_slots);
+/* cerb_batch_marginalize with the new prior kept on the device as the prior of the same window at the next cerb_resident_upload (block
+ * indices already shifted to the next window).  valid [n]: whether window w has a prior afterwards (MARGIN_SECOND_NEW without an old prior
+ * keeps none, MARGIN_OLD with nothing dropped invalidates, as MarginalizationInfo::valid does). */
+int cerb_resident_marginalize(CerbHandle *h, const int32_t *flags, const CerbWindowState *states, int32_t *valid);
+/* Seed or replace the prior of one window from the host (prior->valid == 0 removes it). */
+int cerb_resident_set_prior(CerbHandle *h, int32_t window, const CerbPrior *prior);
+/* Read one window's store back as ordinary CerbWindowDesc content (tests, debugging): obs [max_obs] slot by slot; preint or imu_preint
+ * [CERB_WINDOW_SIZE] by preintegration slot, the members an upload carries filled in and the others zero (pass the one that matches use_leg,
+ * NULL for the other); prior with linearized_jacobians / linearized_residuals pointing at storage for CERB_MAX_PRIOR_DIM^2 / CERB_MAX_PRIOR_DIM
+ * doubles.  Any output may be NULL. */
+int cerb_resident_read_window(CerbHandle *h, int32_t window, CerbObservation *obs, CerbIMULegPreint *preint, CerbIMUPreint *imu_preint,
+                              CerbPrior *prior);
+/* Bytes the handle has been asked to move between host and device since cerb_create, and the number of copy operations issued, summed where
+ * the copies are issued: every host-to-device copy, and the device-to-host copies of the entry points a replay uses (download, the per-feature
+ * steps, marginalization, preintegration, the resident group).  The factor-family evaluators' and debug probes' read-backs and copies within
+ * the device are not counted. */
+int cerb_traffic(CerbHandle *h, int64_t *h2d_bytes, int64_t *d2h_bytes, int64_t *dma_ops);
+
 /* ---- sequence replay: the reference's steady-state frame loop for B robots in lock step, host side in C++ inside this library -----------------
  * (csrc/replay_host.inl mirrors Estimator::processIMULeg / processImage (NON_LINEAR) / optimization / slideWindow and FeatureManager,
  * estimator.cpp:590-846,1054-1677, feature_manager.cpp; every numerical step is one of the batched entry points above).  The reference's
@@ -437,6 +492,20 @@ int cerb_replay_feature_ids(CerbReplay *r, int32_t robot, int32_t *n, int32_t *i
 int cerb_replay_flags(CerbReplay *r, int32_t robot, int32_t *n, int32_t *flags, int32_t max_flags);
 /* seconds spent in: preintegrate, triangulate, solve, marginalize, outliers, shift (device + ABI) and in host bookkeeping */
 int cerb_replay_timing(CerbReplay *r, double *device6, double *host);
+/* resident = 1: the replay keeps every robot's window on the device (cerb_resident_*) and cerb_replay_step sends the frame's edits instead
+ * of three full uploads; the trajectories are bit-identical to the default mode.  To be called before the first cerb_replay_seed_frame; the
+ * handle needs max_obs >= 2 * max_features of the replay * CERB_NUM_FRAMES (one slot per live track).  The replay's long-lived host arrays
+ * are registered with the handle (cerb_register_host_buffer) until cerb_replay_destroy. */
+int cerb_replay_set_resident(CerbReplay *r, int32_t resident);
+/* what cerb_replay_step has asked the library to move so far (see cerb_traffic) and the bytes of it that went through staging memcpy */
+int cerb_replay_traffic(CerbReplay *r, int64_t *h2d_bytes, int64_t *d2h_bytes, int64_t *dma_ops, int64_t *staged_bytes);
+/* The window of one robot as the replay would upload it for a per-feature step (every track, in list order), for tests and debugging.
+ * desc points into the replay's own arrays (valid until the next call on r): in the default mode tracks, observations, the preintegration
+ * records and the prior; in resident mode the tracks only (obs_offset = slot * CERB_NUM_FRAMES) and prior.valid.  ids [<= max_ids] feature
+ * ids; preint_current [CERB_WINDOW_SIZE]: 1 where the record of interval i -> i + 1 is up to date (0: samples were added since);
+ * pre_slots [CERB_WINDOW_SIZE]: resident mode's slot of that interval. */
+int cerb_replay_window(CerbReplay *r, int32_t robot, CerbWindowDesc *desc, int32_t *ids, int32_t max_ids, int32_t *preint_current,
+                       int32_t *pre_slots);
 
 /* ---- host-side helpers that stay on the CPU in the reference too ---------------------------- */
 /* Gauge re-anchoring of Estimator::double2vector (estimator.cpp:903-957): rotates the solved

@@ -123,3 +123,50 @@ int cerb_binding_marginalize(EstimatorSeam &e, int marginalization_flag /* MARGI
     const int32_t flag = marginalization_flag;
     return cerb_batch_marginalize(e.gpu_backend, &flag, &s, next_prior, nullptr);
 }
+
+// ---- resident variant: the window stays on the device across frames (cerb_resident_*), the estimator sends each frame's edits ---------------
+// Set up once after cerb_binding_create with cerb_resident_start(e.gpu_backend, 1, 1).  The binding then mirrors what FeatureManager does to
+// feature_per_frame: a cerb_resident_put_observations record per push_back in addFeatureCheckParallax (feature_manager.cpp:93-113), a
+// cerb_resident_edit_tracks record per erase in removeBackShiftDepth / removeBack / removeFront (:450-529), and preintegrates the new
+// interval into the slot of the one slideWindow dropped (cerb_resident_preintegrate).  `slot_of[k]` is the track slot the binding gave the k-th
+// entry of f_manager.feature; `pre_slots[i]` is the slot of il_pre_integrations[i + 1].
+int cerb_binding_optimization_resident(EstimatorSeam &e, const std::vector<int> &slot_of, const int32_t pre_slots[WINDOW_SIZE], CerbSolveReport *rep) {
+    CerbWindowDesc d; std::memset(&d, 0, sizeof(d));
+    e.gpu_features.clear();
+    size_t k = 0;
+    for (auto &it_per_id : e.f_manager->feature) {                    // the walk of estimator.cpp:1173-1216: only the track list travels
+        const size_t at = k++;
+        it_per_id.used_num = it_per_id.feature_per_frame.size();
+        if (it_per_id.used_num < 4) continue;
+        if (at >= slot_of.size() || slot_of[at] < 0) return CERB_ERR_BAD_ARGUMENT;
+        const int slot = slot_of[at];
+        CerbFeature f; f.start_frame = it_per_id.start_frame; f.n_obs = (int)it_per_id.feature_per_frame.size(); f.obs_offset = slot * CERB_NUM_FRAMES; f.reserved = 0;
+        e.gpu_features.push_back(f);
+    }
+    d.n_features = (int32_t)e.gpu_features.size(); d.features = e.gpu_features.data();
+    if (ESTIMATE_EXTRINSIC && e.frame_count == WINDOW_SIZE && e.Vs[0].norm() > 0.2) e.openExEstimation = true;
+    d.extrinsic_open = (ESTIMATE_EXTRINSIC && e.openExEstimation) ? 1 : 0;
+    d.td_open = (ESTIMATE_TD && e.Vs[0].norm() >= 0.2) ? 1 : 0;
+    CerbWindowState s; std::memset(&s, 0, sizeof(s));
+    std::memcpy(s.para_Pose, e.para_Pose, sizeof(s.para_Pose)); std::memcpy(s.para_SpeedBias, e.para_SpeedBias, sizeof(s.para_SpeedBias));
+    std::memcpy(s.para_LegBias, e.para_LegBias, sizeof(s.para_LegBias)); std::memcpy(s.para_Ex_Pose, e.para_Ex_Pose, sizeof(s.para_Ex_Pose));
+    s.para_Td[0] = e.para_Td[0][0]; s.para_Feature = &e.para_Feature[0][0];
+    int rc = cerb_resident_upload(e.gpu_backend, 1, &d, &s, pre_slots); if (rc != CERB_OK) return rc;
+    rc = cerb_batch_solve_resident(e.gpu_backend); if (rc != CERB_OK) return rc;
+    rc = cerb_batch_download(e.gpu_backend, &s, rep);
+    if (rc != CERB_OK && rc != CERB_ERR_NON_FINITE) return rc;
+    std::memcpy(e.para_Pose, s.para_Pose, sizeof(s.para_Pose)); std::memcpy(e.para_SpeedBias, s.para_SpeedBias, sizeof(s.para_SpeedBias));
+    std::memcpy(e.para_LegBias, s.para_LegBias, sizeof(s.para_LegBias)); std::memcpy(e.para_Ex_Pose, s.para_Ex_Pose, sizeof(s.para_Ex_Pose));
+    e.para_Td[0][0] = s.para_Td[0];
+    return rc;
+}
+
+// cerb_binding_marginalize with the new prior left on the device as the prior of the next cerb_resident_upload: nothing but *prior_valid returns
+int cerb_binding_marginalize_resident(EstimatorSeam &e, int marginalization_flag, int32_t *prior_valid) {
+    CerbWindowState s; std::memset(&s, 0, sizeof(s));
+    std::memcpy(s.para_Pose, e.para_Pose, sizeof(s.para_Pose)); std::memcpy(s.para_SpeedBias, e.para_SpeedBias, sizeof(s.para_SpeedBias));
+    std::memcpy(s.para_LegBias, e.para_LegBias, sizeof(s.para_LegBias)); std::memcpy(s.para_Ex_Pose, e.para_Ex_Pose, sizeof(s.para_Ex_Pose));
+    s.para_Td[0] = e.para_Td[0][0]; s.para_Feature = &e.para_Feature[0][0];
+    const int32_t flag = marginalization_flag;
+    return cerb_resident_marginalize(e.gpu_backend, &flag, &s, prior_valid);
+}
