@@ -87,10 +87,16 @@ struct CerbHandle {
     std::vector<std::pair<char *, size_t>> arena; size_t arena_chunk = 0, arena_used = 0;
     Traffic traffic;                  // host <-> device copies issued since cerb_create
     // resident sliding window (cerb_resident_*): robs / rpre / the prior of windows [0, res_n) are edited in place instead of uploaded
+    // Per window of the store: robs, rpre, the prior inside rdesc, prior_J, prior_r, res_extent, res_prior_valid.  Per row of the batch the
+    // last resident upload named (cerb_resident_upload_windows: row i reads store window res_win[i]): everything else.
     int res_n = 0; bool res_leg = true;
-    Resident<int> pre_slot;           // [B][CERB_WINDOW_SIZE] row of rpre that holds interval i -> i + 1
+    Resident<int> pre_slot;           // one copy per upload of n rows: [n][CERB_WINDOW_SIZE] row of rpre that holds interval i -> i + 1, then [n] res_win
+    std::vector<int> res_win;         // [n] store window of each batch row
     std::vector<int> res_extent;      // [B] observations of robs a pack has to read: up to the highest slot ever put
     std::vector<char> res_prior_valid;
+    Resident<double> step_J, step_r;  // the priors of a compact batch by row (prior_gather_kernel; allocated with the first one)
+    bool prior_gathered = false;      // the batch reads its priors from step_J / step_r instead of prior_J / prior_r
+    bool prior_gather_due = false;    // ... and they have not been gathered yet (the per-feature passes read no prior: only a solve or a marginalization gathers)
     std::vector<unsigned char> res_mark;      // [B][O] scratch of the duplicate checks of put / edit (all zero between calls)
 };
 
@@ -202,7 +208,7 @@ static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDev
     CUDA_TRY(alloc(h, h->state, ST_STRIDE)); CUDA_TRY(alloc(h, h->state0, ST_STRIDE)); CUDA_TRY(alloc(h, h->lam, F)); CUDA_TRY(alloc(h, h->lam0, F)); CUDA_TRY(alloc(h, h->rep_d, 2));
     CUDA_TRY(dmalloc(h, &h->d_ws, (size_t)CerbHandle::LANES * h->grid * h->ws_stride)); CUDA_TRY(dmalloc(h, &h->d_dbg, 2 * (NR + F) + 8)); CUDA_TRY(dmalloc(h, &h->d_G, 4));
     CUDA_TRY(dmalloc(h, &h->d_probe_repi, 4)); CUDA_TRY(dmalloc(h, &h->d_probe_repd, 2)); CUDA_TRY(hmalloc(h, &h->h_dbg, 2 * (NR + F) + 8));
-    CUDA_TRY(alloc(h, h->pre_slot, CERB_WINDOW_SIZE, true));
+    CUDA_TRY(alloc(h, h->pre_slot, CERB_WINDOW_SIZE + 1, true));
     h->nfeat.assign(h->B, 0); h->n0.assign(h->B, 0); h->res_extent.assign(h->B, 0); h->res_prior_valid.assign(h->B, 0);
     CUDA_TRY(cudaMemcpy(h->d_G, cfg->g, 3 * sizeof(double), cudaMemcpyHostToDevice));
     return CERB_OK;
@@ -363,7 +369,7 @@ static int run_plan(CerbHandle *h, const UploadPlan &pl, cudaStream_t s, double 
 // validate windows [w0, w0 + cn), move their raw descriptors to the device on stream s (staging only what is not registered)
 static int upload_raw(CerbHandle *h, int w0, int cn, const CerbWindowDesc *descs, const CerbWindowState *states, cudaStream_t s, double *t_stage_ms) {
     for (int w = w0; w < w0 + cn; w++) { int rc = validate_window(h, descs[w], states[w], &h->n0[w]); if (rc) return rc; h->nfeat[w] = descs[w].n_features; }
-    h->res_n = 0;                      // robs / rpre / the prior are overwritten: the resident sliding window, if there was one, is gone
+    h->res_n = 0; h->prior_gathered = h->prior_gather_due = false;       // robs / rpre / the prior are overwritten: the resident sliding window, if there was one, is gone
     UploadPlan pl;
     plan_rows(h, pl, w0, cn, h->rdesc, 0, 1, 0, [&](int w) { return (const void *)&descs[w]; }, [&](int) { return sizeof(CerbWindowDesc); });
     plan_rows(h, pl, w0, cn, h->rstate, 0, 1, 0, [&](int w) { return (const void *)&states[w]; }, [&](int) { return sizeof(CerbWindowState); });
@@ -399,7 +405,7 @@ static int enqueue_pack(CerbHandle *h, int w0, int cn, cudaStream_t s) {
     P.n_features = h->n_features.at(w0); P.feat_start = h->feat_start.at(w0); P.feat_nobs = h->feat_nobs.at(w0); P.feat_off = h->feat_off.at(w0); P.flags = h->flags.at(w0);
     P.obs_stereo = h->obs_stereo.at(w0); P.prior_meta = h->prior_meta.at(w0); P.perm = h->perm.at(w0);
     P.obs = h->obs.at(w0); P.pre = h->pre.at(w0); P.prior_x0 = h->prior_x0.at(w0); P.state0 = h->state0.at(w0); P.lam0 = h->lam0.at(w0);
-    if (h->res_n) P.pre_slot = h->pre_slot.at(w0);
+    if (h->res_n) { P.pre_slot = h->pre_slot.d; P.window = h->pre_slot.d + (size_t)cn * CERB_WINDOW_SIZE; }      // a resident batch is packed whole (w0 = 0)
     CERB_LAUNCH(pack_kernel, std::min(cn, 8 * h->sm_count), PACK_THREADS, 0, s, P);
     CUDA_TRY(cudaGetLastError());
     return CERB_OK;
@@ -421,6 +427,10 @@ static int ensure_perm(CerbHandle *h) {
     return CERB_OK;
 }
 
+// the prior matrices and residuals of the batch by row: the store, or the per-step copy of a compact batch of resident windows
+static const Resident<double> &batch_prior_J(const CerbHandle *h) { return h->prior_gathered ? h->step_J : h->prior_J; }
+static const Resident<double> &batch_prior_r(const CerbHandle *h) { return h->prior_gathered ? h->step_r : h->prior_r; }
+
 static SolveParams make_params(CerbHandle *h, int w0, int n, int max_iters, double *dbg, int dbg_window) {
     SolveParams P;
     std::memset(&P, 0, sizeof(P));
@@ -432,7 +442,7 @@ static SolveParams make_params(CerbHandle *h, int w0, int n, int max_iters, doub
     P.min_rel_dec = c.min_relative_decrease; P.ftol = c.function_tolerance; P.gtol = c.gradient_tolerance; P.ptol = c.parameter_tolerance;
     P.n_features = h->n_features.at(w0); P.feat_start = h->feat_start.at(w0); P.feat_nobs = h->feat_nobs.at(w0); P.feat_off = h->feat_off.at(w0); P.flags = h->flags.at(w0);
     P.obs = h->obs.at(w0); P.obs_stereo = h->obs_stereo.at(w0); P.pre = h->pre.at(w0); P.sinfo = h->sinfo.at(w0);
-    P.prior_J = h->prior_J.at(w0); P.prior_r = h->prior_r.at(w0); P.prior_x0 = h->prior_x0.at(w0); P.prior_Hp = h->prior_Hp.at(w0); P.prior_meta = h->prior_meta.at(w0);
+    P.prior_J = batch_prior_J(h).at(w0); P.prior_r = batch_prior_r(h).at(w0); P.prior_x0 = h->prior_x0.at(w0); P.prior_Hp = h->prior_Hp.at(w0); P.prior_meta = h->prior_meta.at(w0);
     P.state = h->state.at(w0); P.lam = h->lam.at(w0); P.rep_i = h->rep_i.at(w0); P.rep_d = h->rep_d.at(w0); P.ws = h->d_ws; P.ws_stride = h->ws_stride;
     P.dbg = dbg; P.dbg_window = dbg_window;
     P.test_fail_factorizations = h->test_fail_factorizations; P.test_initial_mu = h->test_initial_mu;
@@ -444,7 +454,18 @@ static SolveParams make_params(CerbHandle *h, int w0, int n, int max_iters, doub
 static void enqueue_prepare(CerbHandle *h, int w0, int n, cudaStream_t s) {
     const int nfac = n * CERB_WINDOW_SIZE;
     CERB_LAUNCH(imu_leg_prepare_kernel, (nfac + 1) / 2, 64, 0, s, nfac, (const double *)h->pre.at(w0), h->sinfo.at(w0));
-    CERB_LAUNCH(prior_prepare_kernel, n, 256, (size_t)PRIOR_TROWS * PRIOR_TLD * sizeof(double), s, (const double *)h->prior_J.at(w0), (const int *)h->prior_meta.at(w0), h->prior_Hp.at(w0));
+    CERB_LAUNCH(prior_prepare_kernel, n, 256, (size_t)PRIOR_TROWS * PRIOR_TLD * sizeof(double), s, (const double *)batch_prior_J(h).at(w0), (const int *)h->prior_meta.at(w0), h->prior_Hp.at(w0));
+}
+
+// a compact batch of resident windows: the listed windows' priors into the per-step area, once per upload, on stream s
+static int gather_priors(CerbHandle *h, cudaStream_t s) {
+    if (!h->prior_gather_due) return CERB_OK;
+    const int n = h->n;
+    CERB_LAUNCH(prior_gather_kernel, std::min(n, 8 * h->sm_count), 256, 0, s, n, (const int *)(h->pre_slot.d + (size_t)n * CERB_WINDOW_SIZE), (const CerbWindowDesc *)h->rdesc.d,
+                (const double *)h->prior_J.d, (const double *)h->prior_r.d, h->step_J.d, h->step_r.d);
+    CUDA_TRY(cudaGetLastError());
+    h->prior_gather_due = false;
+    return CERB_OK;
 }
 
 // restore the initial states of windows [w0, w0 + n), prepare (sqrt_info, prior Gram matrix) and solve; asynchronous on the stream
@@ -454,6 +475,7 @@ static int enqueue_solve(CerbHandle *h, int w0, int n, int max_iters, double *db
         CUDA_TRY(cudaMemcpyAsync(h->state.at(w0), h->state0.at(w0), h->state.bytes(n), cudaMemcpyDeviceToDevice, s));
         CUDA_TRY(cudaMemcpyAsync(h->lam.at(w0), h->lam0.at(w0), h->lam.bytes(n), cudaMemcpyDeviceToDevice, s));
     }
+    int rc = gather_priors(h, s); if (rc) return rc;
     enqueue_prepare(h, w0, n, s);
     SolveParams P = make_params(h, w0, n, max_iters, dbg, dbg_window);
     P.ws = h->d_ws + (size_t)lane * h->grid * h->ws_stride;                      // kernels of different lanes run concurrently: one workspace slice each
@@ -999,6 +1021,7 @@ static int marginalize_impl(CerbHandle *h, const int32_t *flags, const CerbWindo
     if (!dflags || !ddims || !dblocks || !dsw || !dJ || !dr || !dA || !db || !dws) return fail(CERB_ERR_CUDA, "device allocation failed");
     CUDA_TRY(cudaMemsetAsync(dsw, 0, (size_t)n * 2 * sizeof(int), s));
     CUDA_TRY(cudaFuncSetAttribute(marg_assemble_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_bytes));
+    int rc = gather_priors(h, s); if (rc) return rc;
     for (int w0 = 0; w0 < n; w0 += per) {
         const int cn = std::min(per, n - w0);
         enqueue_prepare(h, w0, cn, s);         // a solve leaves sqrt_info and the prior's Gram matrix behind; a bare upload does not
@@ -1017,13 +1040,14 @@ static int marginalize_impl(CerbHandle *h, const int32_t *flags, const CerbWindo
         COPY_TRY(h, hdims.data(), ddims, hdims.size() * sizeof(int), cudaMemcpyDeviceToHost, s);
         CUDA_TRY(cudaStreamSynchronize(s));
         for (int w = 0; w < n; w++) if (hdims[4 * w + 2] == 1 && (hdims[4 * w] > mmax || hdims[4 * w + 1] > nmax)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_resident_marginalize: a window exceeds the structural size of the kept / dropped blocks");
-        CERB_LAUNCH(prior_handover_kernel, std::min(n, 8 * h->sm_count), 256, 0, s, n, (const int *)ddims, (const int *)dblocks, (const double *)lin.state.d, (const double *)dJ, (long)jper,
-                    (const double *)dr, (long)rper, h->rdesc.d, h->prior_J.d, h->prior_r.d);
+        CERB_LAUNCH(prior_handover_kernel, std::min(n, 8 * h->sm_count), 256, 0, s, n, (const int *)(h->pre_slot.d + (size_t)n * CERB_WINDOW_SIZE), (const int *)ddims, (const int *)dblocks,
+                    (const double *)lin.state.d, (const double *)dJ, (long)jper, (const double *)dr, (long)rper, h->rdesc.d, h->prior_J.d, h->prior_r.d);
         CUDA_TRY(cudaGetLastError());
         for (int w = 0; w < n; w++) {
             const int status = hdims[4 * w + 2];
-            if (status != 2) h->res_prior_valid[w] = status == 1;
-            valid[w] = h->res_prior_valid[w];
+            char &v = h->res_prior_valid[h->res_win[w]];
+            if (status != 2) v = status == 1;
+            valid[w] = v;
         }
         return CERB_OK;
     }
@@ -1050,8 +1074,8 @@ static int marginalize_impl(CerbHandle *h, const int32_t *flags, const CerbWindo
         if (status == 2) {                       // MARGIN_SECOND_NEW without para_Pose[WINDOW_SIZE - 1] in the old prior: unchanged (estimator.cpp:1380-1381)
             decode_prior(hmeta.data() + w * h->prior_meta.per, hx0.data() + w * h->prior_x0.per, pr);
             if (!pr.valid) continue;
-            COPY_TRY(h, Jout, h->prior_J.at(w), (size_t)pr.n * pr.n * 8, cudaMemcpyDeviceToHost, s);
-            COPY_TRY(h, rout, h->prior_r.at(w), (size_t)pr.n * 8, cudaMemcpyDeviceToHost, s);
+            COPY_TRY(h, Jout, batch_prior_J(h).at(w), (size_t)pr.n * pr.n * 8, cudaMemcpyDeviceToHost, s);
+            COPY_TRY(h, rout, batch_prior_r(h).at(w), (size_t)pr.n * 8, cudaMemcpyDeviceToHost, s);
             continue;
         }
         const int nn = hdims[4 * w + 1], nb = hdims[4 * w + 3];

@@ -24,6 +24,9 @@ struct PackParams {
     int *n_features, *feat_start, *feat_nobs, *feat_off, *flags, *obs_stereo, *prior_meta, *perm;
     double *obs, *pre, *prior_x0, *state0, *lam0;
     const int *pre_slot = nullptr;       // [n][CERB_WINDOW_SIZE] row of rpre that holds interval i -> i + 1 (resident sliding window); null: row i
+    // [n] store window of batch row w (a compact batch of resident windows): robs, rpre and the prior inside rdesc are read at window[w],
+    // everything else (the descriptor's head and tail, rfeat, rstate, rlam and every output) at w; null: window w
+    const int *window = nullptr;
 };
 
 CERB_HD double pack_pre_leg(const double *raw, int k) {
@@ -81,6 +84,7 @@ CERB_GLOBAL void __launch_bounds__(PACK_THREADS) pack_kernel(CERB_GRID_CONSTANT 
     const int tid = threadIdx.x;
     for (int w = blockIdx.x; w < P.n; w += gridDim.x) {
         const CerbWindowDesc &d = P.rdesc[w];
+        const int sw = P.window ? P.window[w] : w;                   // the window of the store this row reads
         const int F = P.maxF, O = P.maxObs, nF = d.n_features, nO = d.n_obs;
         const bool leg = d.preint != nullptr;                        // host pointer value: only its null-ness is used
         const CerbFeature *ft = P.rfeat + (size_t)w * F;
@@ -105,7 +109,7 @@ CERB_GLOBAL void __launch_bounds__(PACK_THREADS) pack_kernel(CERB_GRID_CONSTANT 
         if (tid == 0) { P.n_features[w] = nF; P.flags[w] = (d.extrinsic_open ? 1 : 0) | (d.td_open ? 2 : 0) | (leg ? 0 : 4); }
         // ---- observations: AoS -> planes ----------------------------------------------------------------------------
         {
-            const CerbObservation *ob = P.robs + (size_t)w * O;
+            const CerbObservation *ob = P.robs + (size_t)sw * O;
             double *op = P.obs + (size_t)w * NOBS_PLANES * O;
             int *so = P.obs_stereo + (size_t)w * O;
             for (int o = tid; o < nO; o += PACK_THREADS) {
@@ -118,13 +122,13 @@ CERB_GLOBAL void __launch_bounds__(PACK_THREADS) pack_kernel(CERB_GRID_CONSTANT 
         // ---- preintegration records ----------------------------------------------------------------------------------
         for (int e = tid; e < CERB_WINDOW_SIZE * PRE_STRIDE; e += PACK_THREADS) {
             const int i = e / PRE_STRIDE, k = e % PRE_STRIDE;
-            const double *raw = P.rpre + ((size_t)w * CERB_WINDOW_SIZE + (P.pre_slot ? P.pre_slot[w * CERB_WINDOW_SIZE + i] : i)) * RAW_PRE_STRIDE;
+            const double *raw = P.rpre + ((size_t)sw * CERB_WINDOW_SIZE + (P.pre_slot ? P.pre_slot[w * CERB_WINDOW_SIZE + i] : i)) * RAW_PRE_STRIDE;
             P.pre[((size_t)w * CERB_WINDOW_SIZE + i) * PRE_STRIDE + k] = leg ? pack_pre_leg(raw, k) : pack_pre_imu(raw, k);
         }
         // ---- prior block list -----------------------------------------------------------------------------------------
         {
             int *meta = P.prior_meta + (size_t)w * PRIOR_META_STRIDE;
-            const CerbPrior &pr = d.prior;
+            const CerbPrior &pr = P.rdesc[sw].prior;
             for (int k = tid; k < PRIOR_META_STRIDE; k += PACK_THREADS) {
                 int v = 0;
                 if (pr.valid) {

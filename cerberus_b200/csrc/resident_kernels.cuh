@@ -65,13 +65,15 @@ CERB_GLOBAL void preint_store_kernel(int n, int imu_only, const int *where, cons
 
 // After marg_schur_kernel has finished: window w's new prior (dims / blocks of marg_assemble_kernel, x0 from the states it linearised at,
 // J / r from the Schur kernel's output) replaces the old one, which was an input of those kernels.  status 2 (carried over) leaves it alone,
-// status 0 (MARGIN_OLD with nothing dropped) invalidates it.
-CERB_GLOBAL void prior_handover_kernel(int n, const int *dims, const int *blocks, const double *state, const double *J, long j_stride, const double *r, long r_stride,
-                                       CerbWindowDesc *rdesc, double *prior_J, double *prior_r) {
+// status 0 (MARGIN_OLD with nothing dropped) invalidates it.  window [n] (a compact batch): row w's prior goes to store window window[w];
+// null: to window w.
+CERB_GLOBAL void prior_handover_kernel(int n, const int *window, const int *dims, const int *blocks, const double *state, const double *J, long j_stride, const double *r,
+                                       long r_stride, CerbWindowDesc *rdesc, double *prior_J, double *prior_r) {
     for (int w = blockIdx.x; w < n; w += gridDim.x) {
         const int status = dims[4 * w + 2], nn = dims[4 * w + 1], nb = dims[4 * w + 3];
+        const int sw = window ? window[w] : w;
         if (status == 2) continue;
-        CerbPrior &pr = rdesc[w].prior;
+        CerbPrior &pr = rdesc[sw].prior;
         if (status == 0) { if (threadIdx.x == 0) pr.valid = 0; continue; }
         if (threadIdx.x == 0) { pr.valid = 1; pr.n = nn; pr.num_blocks = nb; pr.reserved = 0; }
         if (threadIdx.x < CERB_MAX_PRIOR_BLOCKS) {
@@ -83,7 +85,23 @@ CERB_GLOBAL void prior_handover_kernel(int n, const int *dims, const int *blocks
             for (int k = 0; k < 9; k++) pr.block_x0[b][k] = k < size ? x[k] : 0.0;
         }
         const double *Js = J + (size_t)w * j_stride, *rs = r + (size_t)w * r_stride;
-        double *Jd = prior_J + (size_t)w * PRIOR_LD * PRIOR_LD, *rd = prior_r + (size_t)w * PRIOR_LD;
+        double *Jd = prior_J + (size_t)sw * PRIOR_LD * PRIOR_LD, *rd = prior_r + (size_t)sw * PRIOR_LD;
+        for (int e = threadIdx.x; e < nn * nn; e += blockDim.x) Jd[e] = Js[e];
+        for (int e = threadIdx.x; e < nn; e += blockDim.x) rd[e] = rs[e];
+    }
+}
+
+// A compact batch of resident windows: the prior matrix and residuals of store window window[w] into row w of a per-step area.  The solve,
+// prior_prepare_kernel and marg_assemble_kernel index the prior by batch row; pointed at this area they read each row's own prior without
+// a change, and the store keeps one prior per window (prior_handover_kernel writes the next one there).
+CERB_GLOBAL void prior_gather_kernel(int n, const int *window, const CerbWindowDesc *rdesc, const double *prior_J, const double *prior_r, double *step_J, double *step_r) {
+    for (int w = blockIdx.x; w < n; w += gridDim.x) {
+        const int sw = window[w];
+        const CerbPrior &pr = rdesc[sw].prior;
+        if (!pr.valid) continue;
+        const int nn = pr.n;
+        const double *Js = prior_J + (size_t)sw * PRIOR_LD * PRIOR_LD, *rs = prior_r + (size_t)sw * PRIOR_LD;
+        double *Jd = step_J + (size_t)w * PRIOR_LD * PRIOR_LD, *rd = step_r + (size_t)w * PRIOR_LD;
         for (int e = threadIdx.x; e < nn * nn; e += blockDim.x) Jd[e] = Js[e];
         for (int e = threadIdx.x; e < nn; e += blockDim.x) rd[e] = rs[e];
     }

@@ -533,8 +533,9 @@ class DeviceOps:
 
 
 class NativeReplay:
-    """The same lock-step replay with the host side in C++ inside the library (csrc/replay_host.inl, cerb_replay_*): one call per camera frame
-    for all robots.  Same inputs and outputs as ReplayDriver(DeviceOps(...)); tests/test_replay.py compares the two."""
+    """The replay with the host side in C++ inside the library (csrc/replay_host.inl, cerb_replay_*): one call per camera frame, for all robots
+    in lock step (same inputs and outputs as ReplayDriver(DeviceOps(...)); tests/test_replay.py compares the two) or for any subset of them,
+    each at its own stamp (step(robots=, headers=)); a robot restarts with reset() + seed_robot() while the others keep stepping."""
 
     def __init__(self, backend, pcfg, n, max_features=160, estimate_extrinsic=1, estimate_td=0, resident=False):
         """resident=True: every robot's window stays on the device across frames (cerb_resident_*) and a step sends the frame's edits
@@ -564,29 +565,47 @@ class NativeReplay:
         return im
 
     def seed(self, seq):
-        L, _p = self.be.lib, lambda a: np.ascontiguousarray(a, dtype=np.float64).ctypes.data_as(abi.c_dp)
         for w in range(self.n):
-            tic, ric = np.ascontiguousarray(seq.tic_g[w]), np.ascontiguousarray(seq.ric_g[w])
-            self.be._check(L.cerb_replay_set_extrinsics(self.r, w, _p(tic), _p(ric)))
-            for k in range(WINDOW_SIZE + 1):
-                keep = []
-                first = np.ascontiguousarray(seq.first[w, 0 if k == 0 else k - 1: (1 if k == 0 else k)])
-                smp = np.ascontiguousarray(seq.samples[w][k - 1]) if k > 0 else first[:0]
-                im = self._image(seq.images[k][w], keep) if k < WINDOW_SIZE else None
-                P, R, V = np.ascontiguousarray(seq.p_g[w, k]), np.ascontiguousarray(seq.R_g[w, k]), np.ascontiguousarray(seq.v_g[w, k])
-                self.be._check(L.cerb_replay_seed_frame(self.r, w, k, _p(P), _p(R), _p(V), first.ctypes.data, smp.ctypes.data if len(smp) else None, len(smp),
-                                                        C.byref(im) if im is not None else None, float(k)))
+            self.seed_robot(w, seq, w)
 
-    def step(self, images, firsts, samples, header):
+    def seed_robot(self, robot, seq, w, k0=0):
+        """Seed robot `robot` with frames k0 .. k0 + WINDOW_SIZE of robot w of seq (stamps k0 + k), at any time: a robot just created or reset
+        while the others keep stepping.  Its first step then takes frame k0 + WINDOW_SIZE's image with an empty interval."""
+        L, _p = self.be.lib, lambda a: np.ascontiguousarray(a, dtype=np.float64).ctypes.data_as(abi.c_dp)
+        tic, ric = np.ascontiguousarray(seq.tic_g[w]), np.ascontiguousarray(seq.ric_g[w])
+        self.be._check(L.cerb_replay_set_extrinsics(self.r, robot, _p(tic), _p(ric)))
+        for k in range(WINDOW_SIZE + 1):
+            keep, K = [], k0 + k
+            first = np.ascontiguousarray(seq.first[w, K if k == 0 else K - 1: (K + 1 if k == 0 else K)])
+            smp = np.ascontiguousarray(seq.samples[w][K - 1]) if k > 0 else first[:0]
+            im = self._image(seq.images[K][w], keep) if k < WINDOW_SIZE else None
+            P, R, V = np.ascontiguousarray(seq.p_g[w, K]), np.ascontiguousarray(seq.R_g[w, K]), np.ascontiguousarray(seq.v_g[w, K])
+            self.be._check(L.cerb_replay_seed_frame(self.r, robot, k, _p(P), _p(R), _p(V), first.ctypes.data, smp.ctypes.data if len(smp) else None, len(smp),
+                                                    C.byref(im) if im is not None else None, float(K)))
+
+    def reset(self, robot):
+        """The reference's estimator restart (clearState) for one robot; it is seeded again (seed_robot) before it steps."""
+        self.be._check(self.be.lib.cerb_replay_reset_robot(self.r, robot))
+
+    def step(self, images, firsts, samples, header, robots=None, headers=None):
+        """One camera frame of every robot at stamp `header`, or of the robots listed in `robots` (each at its own stamp headers[i] if given);
+        images / firsts / samples are in the order of `robots`.  self.reports gets the step's solve reports in that order."""
         keep = []
-        ims = (abi.Image * self.n)(*[self._image(images[w], keep) for w in range(self.n)])
-        fr = np.ascontiguousarray(np.stack([np.asarray(firsts[w]).reshape(()) for w in range(self.n)]))
-        smp = [np.ascontiguousarray(samples[w]) for w in range(self.n)]
-        ptrs = (C.c_void_p * self.n)(*[s.ctypes.data if len(s) else None for s in smp])
-        ns = (C.c_int32 * self.n)(*[len(s) for s in smp])
-        rep = (abi.SolveReport * self.n)()
-        self.be._check(self.be.lib.cerb_replay_step(self.r, ims, fr.ctypes.data, ptrs, ns, float(header), rep))
-        self.reports.append(np.frombuffer(rep, dtype=abi.report_dtype, count=self.n).copy())
+        m = self.n if robots is None else len(robots)
+        ims = (abi.Image * m)(*[self._image(images[i], keep) for i in range(m)])
+        fr = np.ascontiguousarray(np.stack([np.asarray(firsts[i]).reshape(()) for i in range(m)]))
+        smp = [np.ascontiguousarray(samples[i]) for i in range(m)]
+        ptrs = (C.c_void_p * m)(*[s.ctypes.data if len(s) else None for s in smp])
+        ns = (C.c_int32 * m)(*[len(s) for s in smp])
+        rep = (abi.SolveReport * m)()
+        if robots is None and headers is None:
+            self.be._check(self.be.lib.cerb_replay_step(self.r, ims, fr.ctypes.data, ptrs, ns, float(header), rep))
+        else:
+            rob = np.ascontiguousarray(np.arange(self.n) if robots is None else robots, dtype=np.int32)
+            hdr = np.ascontiguousarray(np.full(m, float(header)) if headers is None else headers, dtype=np.float64)
+            self.be._check(self.be.lib.cerb_replay_step_robots(self.r, m, rob.ctypes.data_as(C.POINTER(C.c_int32)), ims, fr.ctypes.data, ptrs, ns,
+                                                               hdr.ctypes.data_as(abi.c_dp), rep))
+        self.reports.append(np.frombuffer(rep, dtype=abi.report_dtype, count=m).copy())
 
     def run(self, seq, n_steps=None):
         self.seed(seq)

@@ -78,6 +78,8 @@ class Backend:
         L.cerb_replay_feature_ids.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
         L.cerb_replay_timing.argtypes = [C.c_void_p, abi.c_dp, abi.c_dp]
         i32p, i64p = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
+        L.cerb_replay_step_robots.argtypes = [C.c_void_p, C.c_int32, i32p, C.POINTER(abi.Image), C.c_void_p, C.POINTER(C.c_void_p), i32p, abi.c_dp, C.POINTER(abi.SolveReport)]
+        L.cerb_replay_reset_robot.argtypes = [C.c_void_p, C.c_int32]
         L.cerb_replay_set_resident.argtypes = [C.c_void_p, C.c_int32]
         L.cerb_replay_traffic.argtypes = [C.c_void_p, i64p, i64p, i64p, i64p]
         L.cerb_replay_window.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.WindowDesc), i32p, C.c_int32, i32p, i32p]
@@ -86,6 +88,7 @@ class Backend:
         L.cerb_resident_edit_tracks.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.TrackEdit)]
         L.cerb_resident_preintegrate.argtypes = [C.c_void_p, C.POINTER(abi.PreintConfig), C.c_int32, C.POINTER(abi.PreintJob), i32p, i32p, abi.c_dp]
         L.cerb_resident_upload.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.WindowDesc), C.POINTER(abi.WindowState), i32p]
+        L.cerb_resident_upload_windows.argtypes = [C.c_void_p, C.c_int32, i32p, C.POINTER(abi.WindowDesc), C.POINTER(abi.WindowState), i32p]
         L.cerb_resident_marginalize.argtypes = [C.c_void_p, i32p, C.POINTER(abi.WindowState), i32p]
         L.cerb_resident_set_prior.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Prior)]
         L.cerb_resident_read_window.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Observation), C.POINTER(abi.IMULegPreint), C.POINTER(abi.IMUPreint), C.POINTER(abi.Prior)]
@@ -264,6 +267,13 @@ class Backend:
         """feature lists (obs_offset = slot * NUM_FRAMES), open flags and states of batch against the resident data; pre_slots [n, 10]"""
         ps = np.ascontiguousarray(np.tile(np.arange(abi.WINDOW_SIZE), (batch.n, 1)) if pre_slots is None else pre_slots, dtype=np.int32)
         self._check(self.lib.cerb_resident_upload(self.h, batch.n, batch.descs, batch.states, ps.ctypes.data_as(C.POINTER(C.c_int32))))
+
+    def resident_upload_windows(self, windows, batch, pre_slots=None):
+        """resident_upload of a compact batch: row i of batch (and of pre_slots) is resident window windows[i]"""
+        win = np.ascontiguousarray(windows, dtype=np.int32)
+        ps = np.ascontiguousarray(np.tile(np.arange(abi.WINDOW_SIZE), (len(win), 1)) if pre_slots is None else pre_slots, dtype=np.int32)
+        self._check(self.lib.cerb_resident_upload_windows(self.h, len(win), win.ctypes.data_as(C.POINTER(C.c_int32)), batch.descs, batch.states,
+                                                          ps.ctypes.data_as(C.POINTER(C.c_int32))))
 
     def resident_marginalize(self, flags, states):
         flags = np.ascontiguousarray(flags, dtype=np.int32); valid = np.zeros(len(flags), dtype=np.int32)

@@ -438,6 +438,12 @@ int cerb_resident_preintegrate(CerbHandle *h, const CerbPreintConfig *cfg, int32
  * 0 .. CERB_WINDOW_SIZE - 1 per window.  n must be the n of cerb_resident_start.  Afterwards the resident batch is used as after
  * cerb_batch_upload (cerb_batch_solve_resident, cerb_batch_download, the per-feature steps, cerb_batch_update_states). */
 int cerb_resident_upload(CerbHandle *h, int32_t n, const CerbWindowDesc *descs, const CerbWindowState *states, const int32_t *pre_slots);
+/* cerb_resident_upload of a compact batch of 1 <= n <= (n of cerb_resident_start) rows: row i is resident window windows[i] (no window listed
+ * twice), descs / states / pre_slots are in list order.  The batch calls that follow (cerb_batch_solve_resident, cerb_batch_download,
+ * cerb_batch_update_states, the per-feature steps, cerb_resident_marginalize) work on the n rows; the marginalization leaves each new prior in
+ * window windows[i].  The windows not listed are not touched.  cerb_resident_upload is this call with windows = 0 .. n - 1. */
+int cerb_resident_upload_windows(CerbHandle *h, int32_t n, const int32_t *windows, const CerbWindowDesc *descs, const CerbWindowState *states,
+                                 const int32_t *pre_slots);
 /* cerb_batch_marginalize with the new prior kept on the device as the prior of the same window at the next cerb_resident_upload (block
  * indices already shifted to the next window).  valid [n]: whether window w has a prior afterwards (MARGIN_SECOND_NEW without an old prior
  * keeps none, MARGIN_OLD with nothing dropped invalidates, as MarginalizationInfo::valid does). */
@@ -485,6 +491,18 @@ int cerb_replay_seed_frame(CerbReplay *r, int32_t robot, int32_t k, const double
  * samples [n_robots] pointers / n_samples [n_robots] (the new interval), header = the frame's stamp; reports (optional) [n_robots]. */
 int cerb_replay_step(CerbReplay *r, const CerbImage *images, const CerbIMULegSample *firsts, const CerbIMULegSample *const *samples,
                      const int32_t *n_samples, double header, CerbSolveReport *reports);
+/* processMeasurements for one camera frame of the n_active robots robots[0 .. n_active - 1] only, each at its own stamp: every array is in
+ * list order (images, firsts, samples, n_samples, headers [n_active]; reports, optional, [n_active]).  The robots not listed are not touched,
+ * and the order of the list changes no result.  A robot must be listed at most once and be seeded (frames 0 .. WINDOW_SIZE since its
+ * creation or its last cerb_replay_reset_robot).  A call that is rejected changes nothing and moves nothing.  cerb_replay_step is this call
+ * with every robot, in order, at one stamp. */
+int cerb_replay_step_robots(CerbReplay *r, int32_t n_active, const int32_t *robots, const CerbImage *images, const CerbIMULegSample *firsts,
+                            const CerbIMULegSample *const *samples, const int32_t *n_samples, const double *headers, CerbSolveReport *reports);
+/* Estimator::clearState for one robot (the reference's restart, main.cpp:236-251): its features, intervals, prior, extrinsic latch and frame
+ * count are gone, extrinsics back at the values of cerb_replay_set_extrinsics; in resident mode its track slots are free again, its device
+ * prior is invalid and its preintegration slot table is the identity.  Its path rows and flag history stay.  It is seeded again with
+ * cerb_replay_seed_frame (frames 0 .. WINDOW_SIZE) before it is stepped; the other robots may step meanwhile. */
+int cerb_replay_reset_robot(CerbReplay *r, int32_t robot);
 /* Published states of the newest frame after every processed image: rows of 20 doubles = header, P(3), R(9, row-major), V(3), rho(4). */
 int cerb_replay_path(CerbReplay *r, int32_t robot, int32_t *n_rows, double *out, int32_t max_rows);
 int cerb_replay_feature_ids(CerbReplay *r, int32_t robot, int32_t *n, int32_t *ids, int32_t max_ids);
