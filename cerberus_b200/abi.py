@@ -182,6 +182,15 @@ def default_preint_config():
     return p
 
 
+def vins_preint_config():
+    """The A1 VINS baseline (config/a1_config/hardware_a1_vins_config.yaml: no use_leg_odom, so USE_LEG == 0; acc_n 0.5, gyr_n 0.05,
+    acc_w 0.0004, gyr_w 0.0002).  IntegrationBase reads acc_n (on all three axes), gyr_n, acc_w and gyr_w only; the other fields keep the
+    A1 VILO values of default_preint_config."""
+    p = default_preint_config()
+    p.acc_n = 0.5
+    return p
+
+
 class WindowBatch:
     """Contiguous host storage for `n` sliding windows + the ctypes views the C ABI takes.
 
@@ -190,6 +199,8 @@ class WindowBatch:
       preint   [n, 10]            preint_dtype       prior_J [n, 96*96], prior_r [n, 96]
       states   ctypes array of WindowState           para_Feature [n, max_features]
       descs    ctypes array of WindowDesc (pointers into the arrays above)
+    Every descriptor starts with IMU-leg records (preint); set_kind switches one to IMUFactor records (imu_preint [n, 10], allocated with
+    the first such window), so one batch may mix the two.
     """
 
     def __init__(self, n, max_features, max_obs=None):
@@ -215,12 +226,21 @@ class WindowBatch:
             d.prior.linearized_residuals = self.prior_r[w].ctypes.data_as(c_dp)
             self.states[w].para_Feature = self.para_Feature[w].ctypes.data_as(c_dp)
 
+    def set_kind(self, w, use_leg):
+        """Descriptor w carries IMU-leg preintegrations (use_leg, USE_LEG == 1) or IMUFactor ones (USE_LEG == 0)."""
+        d = self.descs[w]
+        if use_leg:
+            d.preint = self.preint[w].ctypes.data_as(C.POINTER(IMULegPreint)); d.imu_preint = None
+            return
+        if self.imu_preint is None:
+            self.imu_preint = np.zeros((self.n, WINDOW_SIZE), dtype=imu_preint_dtype)
+        d.preint = None
+        d.imu_preint = self.imu_preint[w].ctypes.data_as(C.POINTER(IMUPreint))
+
     def use_imu_only(self):
         """Switch the batch to USE_LEG == 0: descriptors carry IMUFactor preintegrations instead of IMU-leg ones."""
-        self.imu_preint = np.zeros((self.n, WINDOW_SIZE), dtype=imu_preint_dtype)
         for w in range(self.n):
-            self.descs[w].preint = None
-            self.descs[w].imu_preint = self.imu_preint[w].ctypes.data_as(C.POINTER(IMUPreint))
+            self.set_kind(w, False)
 
     # numpy views of the state arrays (no copy): shape [n, ...]
     def state_array(self):

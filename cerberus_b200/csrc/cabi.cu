@@ -87,13 +87,14 @@ struct CerbHandle {
     std::vector<std::pair<char *, size_t>> arena; size_t arena_chunk = 0, arena_used = 0;
     Traffic traffic;                  // host <-> device copies issued since cerb_create
     // resident sliding window (cerb_resident_*): robs / rpre / the prior of windows [0, res_n) are edited in place instead of uploaded
-    // Per window of the store: robs, rpre, the prior inside rdesc, prior_J, prior_r, res_extent, res_prior_valid.  Per row of the batch the
-    // last resident upload named (cerb_resident_upload_windows: row i reads store window res_win[i]): everything else.
-    int res_n = 0; bool res_leg = true;
+    // Per window of the store: robs, rpre, the prior inside rdesc, prior_J, prior_r, res_extent, res_prior_valid, res_leg.  Per row of the
+    // batch the last resident upload named (cerb_resident_upload_windows: row i reads store window res_win[i]): everything else.
+    int res_n = 0;
     Resident<int> pre_slot;           // one copy per upload of n rows: [n][CERB_WINDOW_SIZE] row of rpre that holds interval i -> i + 1, then [n] res_win
     std::vector<int> res_win;         // [n] store window of each batch row
     std::vector<int> res_extent;      // [B] observations of robs a pack has to read: up to the highest slot ever put
     std::vector<char> res_prior_valid;
+    std::vector<char> res_leg;        // [B] record kind of the window's preintegration slots: 1 CerbIMULegPreint, 0 CerbIMUPreint
     Resident<double> step_J, step_r;  // the priors of a compact batch by row (prior_gather_kernel; allocated with the first one)
     bool prior_gathered = false;      // the batch reads its priors from step_J / step_r instead of prior_J / prior_r
     bool prior_gather_due = false;    // ... and they have not been gathered yet (the per-feature passes read no prior: only a solve or a marginalization gathers)
@@ -209,7 +210,7 @@ static int create_impl(CerbHandle *h, const CerbSolverConfig *cfg, const cudaDev
     CUDA_TRY(dmalloc(h, &h->d_ws, (size_t)CerbHandle::LANES * h->grid * h->ws_stride)); CUDA_TRY(dmalloc(h, &h->d_dbg, 2 * (NR + F) + 8)); CUDA_TRY(dmalloc(h, &h->d_G, 4));
     CUDA_TRY(dmalloc(h, &h->d_probe_repi, 4)); CUDA_TRY(dmalloc(h, &h->d_probe_repd, 2)); CUDA_TRY(hmalloc(h, &h->h_dbg, 2 * (NR + F) + 8));
     CUDA_TRY(alloc(h, h->pre_slot, CERB_WINDOW_SIZE + 1, true));
-    h->nfeat.assign(h->B, 0); h->n0.assign(h->B, 0); h->res_extent.assign(h->B, 0); h->res_prior_valid.assign(h->B, 0);
+    h->nfeat.assign(h->B, 0); h->n0.assign(h->B, 0); h->res_extent.assign(h->B, 0); h->res_prior_valid.assign(h->B, 0); h->res_leg.assign(h->B, 1);
     CUDA_TRY(cudaMemcpy(h->d_G, cfg->g, 3 * sizeof(double), cudaMemcpyHostToDevice));
     return CERB_OK;
 }
@@ -1112,32 +1113,38 @@ int cerb_batch_update_states(CerbHandle *h, int32_t n, const CerbWindowState *st
     return CERB_OK;
 }
 
-// ---- leg-contact preintegration ------------------------------------------------------------------------------------
-// where (resident sliding window): [n][2] window, slot -- the results stay in rpre and only sum_dt [n] returns; else out / out_imu receive them
-static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, CerbIMULegPreint *out, CerbIMUPreint *out_imu,
-                             const int *where = nullptr, double *sum_dt = nullptr) {
-    if (!h || !cfg || n < 1 || !jobs || (!out && !out_imu && !where)) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_preintegrate: bad argument");
+// ---- leg-contact and plain IMU preintegration -----------------------------------------------------------------------
+// Job j integrates under cfgs[cfg_of[j]] into the record kind imu_only[j] (0: IMULegIntegrationBase, 1: IntegrationBase), all in one
+// preintegrate_kernel launch.  where (resident sliding window): [n][2] window, slot -- the results stay in rpre and only sum_dt [n] returns;
+// else out[j] / out_imu[j] receive them by kind.  The caller has validated cfg_of and where.
+static int preintegrate_impl(CerbHandle *h, int32_t n_cfg, const CerbPreintConfig *cfgs, int32_t n, const CerbPreintJob *jobs, const int32_t *cfg_of,
+                             const std::vector<int> &imu_only, CerbIMULegPreint *out, CerbIMUPreint *out_imu, const int *where = nullptr, double *sum_dt = nullptr) {
     CERB_DEVICE(h);
-    PreintParams P;
-    P.imu_only = where ? (h->res_leg ? 0 : 1) : (out_imu ? 1 : 0);
-    P.acc_n = cfg->acc_n; P.acc_n_z = cfg->acc_n_z; P.gyr_n = cfg->gyr_n; P.acc_w = cfg->acc_w; P.gyr_w = cfg->gyr_w; P.phi_n = cfg->phi_n; P.dphi_n = cfg->dphi_n;
-    P.rho_c_n = cfg->rho_c_n; P.rho_nc_n = cfg->rho_nc_n; P.v_n_min_xy = cfg->v_n_min_xy; P.v_n_min_z = cfg->v_n_min_z; P.v_n_min = cfg->v_n_min; P.v_n_max = cfg->v_n_max;
-    P.v_n_force_thres_ratio = cfg->v_n_force_thres_ratio; P.v_n_term1_steep = cfg->v_n_term1_steep; P.v_n_term2_var_rescale = cfg->v_n_term2_var_rescale;
-    P.v_n_term3_distance_rescale = cfg->v_n_term3_distance_rescale; P.contact_sensor_type = cfg->contact_sensor_type;
-    for (int l = 0; l < 4; l++) for (int k = 0; k < 4; k++) P.rho_fix[4 * l + k] = cfg->rho_fix[l][k];
-    for (int k = 0; k < 3; k++) P.p_br[k] = cfg->p_br[k];
-    for (int k = 0; k < 9; k++) P.R_br[k] = cfg->R_br[k];
+    std::vector<PreintParams> table((size_t)2 * n_cfg);      // entry 2 c + imu_only: configuration c with the record kind
+    for (int c = 0; c < 2 * n_cfg; c++) {
+        const CerbPreintConfig *cfg = &cfgs[c / 2];
+        PreintParams &P = table[c];
+        std::memset(&P, 0, sizeof(P));
+        P.imu_only = c % 2;
+        P.acc_n = cfg->acc_n; P.acc_n_z = cfg->acc_n_z; P.gyr_n = cfg->gyr_n; P.acc_w = cfg->acc_w; P.gyr_w = cfg->gyr_w; P.phi_n = cfg->phi_n; P.dphi_n = cfg->dphi_n;
+        P.rho_c_n = cfg->rho_c_n; P.rho_nc_n = cfg->rho_nc_n; P.v_n_min_xy = cfg->v_n_min_xy; P.v_n_min_z = cfg->v_n_min_z; P.v_n_min = cfg->v_n_min; P.v_n_max = cfg->v_n_max;
+        P.v_n_force_thres_ratio = cfg->v_n_force_thres_ratio; P.v_n_term1_steep = cfg->v_n_term1_steep; P.v_n_term2_var_rescale = cfg->v_n_term2_var_rescale;
+        P.v_n_term3_distance_rescale = cfg->v_n_term3_distance_rescale; P.contact_sensor_type = cfg->contact_sensor_type;
+        for (int l = 0; l < 4; l++) for (int k = 0; k < 4; k++) P.rho_fix[4 * l + k] = cfg->rho_fix[l][k];
+        for (int k = 0; k < 3; k++) P.p_br[k] = cfg->p_br[k];
+        for (int k = 0; k < 9; k++) P.R_br[k] = cfg->R_br[k];
+    }
     size_t total = 0;
     for (int j = 0; j < n; j++) { if (jobs[j].n_samples < 0 || (jobs[j].n_samples && !jobs[j].samples)) return fail(CERB_ERR_BAD_ARGUMENT, "bad job"); total += jobs[j].n_samples; }
     std::vector<double> hj((size_t)n * PJ_STRIDE), hs(std::max<size_t>(total, 1) * SAMPLE_STRIDE);
-    std::vector<int> hi((size_t)n * 2);
+    std::vector<int> hi((size_t)n * 3);
     size_t off = 0;
     for (int j = 0; j < n; j++) {
         const CerbPreintJob &q = jobs[j];
         double *o = hj.data() + (size_t)j * PJ_STRIDE;
         std::memcpy(o, q.acc_0, 24); std::memcpy(o + 3, q.gyr_0, 24); std::memcpy(o + 6, q.phi_0, 96); std::memcpy(o + 18, q.dphi_0, 96); std::memcpy(o + 30, q.c_0, 32);
         std::memcpy(o + 34, q.linearized_ba, 24); std::memcpy(o + 37, q.linearized_bg, 24); std::memcpy(o + 40, q.linearized_rho, 32);
-        hi[2 * j] = q.n_samples; hi[2 * j + 1] = (int)off;
+        hi[3 * j] = q.n_samples; hi[3 * j + 1] = (int)off; hi[3 * j + 2] = 2 * cfg_of[j] + imu_only[j];
         for (int k = 0; k < q.n_samples; k++) {
             const CerbIMULegSample &m = q.samples[k];
             double *so = hs.data() + (off + k) * SAMPLE_STRIDE;
@@ -1148,13 +1155,17 @@ static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t
     cudaStream_t s = h->stream; DevBuf B(h);
     double *dj = B.up(hj.data(), hj.size(), s), *ds = B.up(hs.data(), hs.size(), s), *dout = B.up(nullptr, (size_t)n * PRE_STRIDE, s), *dfull = B.up(nullptr, (size_t)n * 1922, s);
     int *di = B.upi(hi.data(), hi.size(), s);
-    if (!dj || !ds || !dout || !dfull || !di) return fail(CERB_ERR_CUDA, "device allocation failed");
-    CERB_LAUNCH(preintegrate_kernel, n, 128, 0, s, P, (int)n, (const double *)dj, (const int *)di, (const double *)ds, dout, dfull);
+    PreintParams *dparams = (PreintParams *)B.raw(table.size() * sizeof(PreintParams));
+    if (!dj || !ds || !dout || !dfull || !di || !dparams) return fail(CERB_ERR_CUDA, "device allocation failed");
+    COPY_TRY(h, dparams, table.data(), table.size() * sizeof(PreintParams), cudaMemcpyHostToDevice, s);
+    CERB_LAUNCH(preintegrate_kernel, n, 128, 0, s, (const PreintParams *)dparams, (int)n, (const double *)dj, (const int *)di, (const double *)ds, dout, dfull);
     CUDA_TRY(cudaGetLastError());
     if (where) {
-        int *dwhere = B.upi(where, (size_t)n * 2, s); double *dsum = B.up(nullptr, n, s);
+        std::vector<int> where3((size_t)n * 3);
+        for (int j = 0; j < n; j++) { where3[3 * j] = where[2 * j]; where3[3 * j + 1] = where[2 * j + 1]; where3[3 * j + 2] = imu_only[j]; }
+        int *dwhere = B.upi(where3.data(), where3.size(), s); double *dsum = B.up(nullptr, n, s);
         if (!dwhere || !dsum) return fail(CERB_ERR_CUDA, "device allocation failed");
-        CERB_LAUNCH(preint_store_kernel, n, 128, 0, s, (int)n, P.imu_only, (const int *)dwhere, (const double *)dout, (const double *)dfull, h->rpre.d, dsum);
+        CERB_LAUNCH(preint_store_kernel, n, 128, 0, s, (int)n, (const int *)dwhere, (const double *)dout, (const double *)dfull, h->rpre.d, dsum);
         CUDA_TRY(cudaGetLastError());
         std::vector<double> hsum(n);
         COPY_TRY(h, hsum.data(), dsum, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s);
@@ -1168,7 +1179,7 @@ static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t
     CUDA_TRY(cudaStreamSynchronize(s));
     for (int j = 0; j < n; j++) {
         const double *o = ho.data() + (size_t)j * PRE_STRIDE, *f = hf.data() + (size_t)j * 1922;
-        if (out_imu) {
+        if (imu_only[j]) {
             CerbIMUPreint &r = out_imu[j];
             r.sum_dt = o[PRE_SUM_DT];
             for (int k = 0; k < 3; k++) { r.delta_p[k] = o[PRE_DP + k]; r.delta_v[k] = o[PRE_DV + k]; r.linearized_ba[k] = o[PRE_BA + k]; r.linearized_bg[k] = o[PRE_BG + k]; }
@@ -1186,11 +1197,31 @@ static int preintegrate_impl(CerbHandle *h, const CerbPreintConfig *cfg, int32_t
     return CERB_OK;
 }
 
+// the arguments every preintegration entry point shares: jobs and their configuration indices
+static int check_preint_args(CerbHandle *h, int32_t n_cfg, const CerbPreintConfig *cfgs, int32_t n, const CerbPreintJob *jobs, const int32_t *cfg_of, const char *who) {
+    if (!h || n_cfg < 1 || !cfgs || n < 1 || !jobs || !cfg_of) return fail(CERB_ERR_BAD_ARGUMENT, std::string(who) + ": bad argument");
+    for (int j = 0; j < n; j++) if (cfg_of[j] < 0 || cfg_of[j] >= n_cfg) return fail(CERB_ERR_BAD_ARGUMENT, std::string(who) + ": cfg_of out of range");
+    return CERB_OK;
+}
+
+int cerb_preintegrate_mixed(CerbHandle *h, int32_t n_cfg, const CerbPreintConfig *cfgs, const int32_t *use_leg, int32_t n, const CerbPreintJob *jobs,
+                            const int32_t *cfg_of, CerbIMULegPreint *out, CerbIMUPreint *out_imu) {
+    int rc = check_preint_args(h, n_cfg, cfgs, n, jobs, cfg_of, "cerb_preintegrate"); if (rc) return rc;
+    if (!use_leg) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_preintegrate: bad argument");
+    std::vector<int> imu_only(n);
+    for (int j = 0; j < n; j++) {
+        imu_only[j] = use_leg[cfg_of[j]] ? 0 : 1;
+        if (imu_only[j] ? !out_imu : !out) return fail(CERB_ERR_BAD_ARGUMENT, "cerb_preintegrate: no output array for a job's record kind");
+    }
+    return preintegrate_impl(h, n_cfg, cfgs, n, jobs, cfg_of, imu_only, out, out_imu);
+}
 int cerb_preintegrate_batch(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, CerbIMULegPreint *out) {
-    return preintegrate_impl(h, cfg, n, jobs, out, nullptr);
+    const int32_t leg = 1; const std::vector<int32_t> cfg_of(std::max(n, 0), 0);
+    return cerb_preintegrate_mixed(h, 1, cfg, &leg, n, jobs, cfg_of.data(), out, nullptr);
 }
 int cerb_preintegrate_imu_batch(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, CerbIMUPreint *out) {
-    return preintegrate_impl(h, cfg, n, jobs, nullptr, out);
+    const int32_t leg = 0; const std::vector<int32_t> cfg_of(std::max(n, 0), 0);
+    return cerb_preintegrate_mixed(h, 1, cfg, &leg, n, jobs, cfg_of.data(), nullptr, out);
 }
 
 // ---- host-side gauge re-anchoring: Estimator::double2vector (estimator.cpp:903-957) ----------------------------------

@@ -11,7 +11,7 @@
 
 namespace cerb {
 
-struct PreintParams {   // mirror of CerbPreintConfig (plain doubles so it can be passed by value)
+struct PreintParams {   // mirror of CerbPreintConfig plus the record kind; a launch reads one entry of a table of them per job
     double acc_n, acc_n_z, gyr_n, acc_w, gyr_w, phi_n, dphi_n, rho_c_n, rho_nc_n;
     double v_n_min_xy, v_n_min_z, v_n_min, v_n_max, v_n_force_thres_ratio, v_n_term1_steep, v_n_term2_var_rescale, v_n_term3_distance_rescale;
     int contact_sensor_type;
@@ -20,7 +20,7 @@ struct PreintParams {   // mirror of CerbPreintConfig (plain doubles so it can b
 };
 
 // device job table: per job [0..2] acc_0 [3..5] gyr_0 [6..17] phi_0 [18..29] dphi_0 [30..33] c_0
-//                   [34..36] lin_ba [37..39] lin_bg [40..43] lin_rho ; n_samples, sample offset in ints
+//                   [34..36] lin_ba [37..39] lin_bg [40..43] lin_rho ; n_samples, sample offset, entry of the parameter table in ints
 enum { PJ_STRIDE = 44, SAMPLE_STRIDE = 35 };   // sample: dt, acc3, gyr3, phi12, dphi12, c4
 enum { NO_Ai = 0, NO_Gi = 3, NO_Ai1 = 6, NO_Gi1 = 9, NO_BA = 12, NO_BG = 15, NO_PHIi = 18, NO_PHIi1 = 21, NO_DPHIi = 24, NO_DPHIi1 = 27, NO_V1 = 30, NO_NRHO1 = 42 };
 
@@ -36,8 +36,9 @@ CERB_D m33 colmajor33(const double *a) { m33 r; for (int c = 0; c < 3; c++) for 
 
 // out (compact device preint layout, PRE_STRIDE doubles): nominal + jacobian sub-blocks + covariance;
 // out_full (optional, 2*961 doubles): full jacobian and covariance, row-major (for the host ABI struct).
-// grid = n_jobs, block = 128.
-CERB_GLOBAL void preintegrate_kernel(PreintParams P, int n_jobs, const double *jobs, const int *job_samples, const double *samples,
+// job_ints [n_jobs][3] = n_samples, sample offset, p: job j integrates under params[p], so one launch serves jobs of several configurations
+// and of both record kinds.  grid = n_jobs, block = 128.
+CERB_GLOBAL void preintegrate_kernel(const PreintParams *params, int n_jobs, const double *jobs, const int *job_ints, const double *samples,
                                      double *out, double *out_full) {
     const int LD = 33, LDV = 47;
     __shared__ double jac[31 * 33], cov[31 * 33], F[31 * 33], T[31 * 33], V[31 * 47], Nn[48];
@@ -48,8 +49,9 @@ CERB_GLOBAL void preintegrate_kernel(PreintParams P, int n_jobs, const double *j
     __shared__ double filt[4 * 12];     // type-2 contact filter state per leg: min, max, thr, var, idx, window[5]
     __shared__ int flag[4];
     const int job = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+    const PreintParams &P = params[job_ints[3 * job + 2]];
     const double *jb = jobs + (size_t)job * PJ_STRIDE;
-    const int n_samples = job_samples[2 * job], s_off = job_samples[2 * job + 1];
+    const int n_samples = job_ints[3 * job], s_off = job_ints[3 * job + 1];
 
     for (int i = tid; i < 31 * 33; i += nt) { const int r = i / 33, c = i % 33; jac[i] = (r == c) ? 1.0 : 0.0; cov[i] = 0.0; }
     if (tid < 34) cur[tid] = jb[tid];

@@ -29,13 +29,15 @@ CERB_GLOBAL void track_edit_kernel(int count, const CerbTrackEdit *edits, CerbOb
 }
 
 // Job j of a preintegrate_kernel launch (packed: [n][PRE_STRIDE], full: [n][1922] = jacobian | covariance, row-major 31 x 31) into slot
-// where[2 j + 1] of window where[2 j].  leg: head (33 doubles in struct order) | jacobian columns 21..30 | covariance, column-major;
-// imu only: the CerbIMUPreint struct (467 doubles), rows / columns P, R, V, BA, BG gathered from their ILStateOrder places.
-CERB_GLOBAL void preint_store_kernel(int n, int imu_only, const int *where, const double *packed, const double *full, double *rpre, double *sum_dt) {
+// where[3 j + 1] of window where[3 j]; where[3 j + 2] is the record kind of that window.  leg (0): head (33 doubles in struct order) |
+// jacobian columns 21..30 | covariance, column-major; imu only (1): the CerbIMUPreint struct (467 doubles), rows / columns P, R, V, BA, BG
+// gathered from their ILStateOrder places.
+CERB_GLOBAL void preint_store_kernel(int n, const int *where, const double *packed, const double *full, double *rpre, double *sum_dt) {
     const int j = blockIdx.x;
     if (j >= n) return;
     const double *o = packed + (size_t)j * PRE_STRIDE, *f = full + (size_t)j * 1922;
-    double *raw = rpre + ((size_t)where[2 * j] * CERB_WINDOW_SIZE + where[2 * j + 1]) * RAW_PRE_STRIDE;
+    double *raw = rpre + ((size_t)where[3 * j] * CERB_WINDOW_SIZE + where[3 * j + 1]) * RAW_PRE_STRIDE;
+    const int imu_only = where[3 * j + 2];
     if (threadIdx.x == 0) sum_dt[j] = o[PRE_SUM_DT];
     if (!imu_only) {
         for (int k = threadIdx.x; k < RAW_PRE_STRIDE; k += blockDim.x) {

@@ -93,6 +93,11 @@ class Backend:
         L.cerb_resident_set_prior.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Prior)]
         L.cerb_resident_read_window.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Observation), C.POINTER(abi.IMULegPreint), C.POINTER(abi.IMUPreint), C.POINTER(abi.Prior)]
         L.cerb_traffic.argtypes = [C.c_void_p, i64p, i64p, i64p]
+        L.cerb_preintegrate_mixed.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.PreintConfig), i32p, C.c_int32, C.POINTER(abi.PreintJob), i32p,
+                                              C.POINTER(abi.IMULegPreint), C.POINTER(abi.IMUPreint)]
+        L.cerb_resident_preintegrate_mixed.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.PreintConfig), C.c_int32, C.POINTER(abi.PreintJob), i32p, i32p, i32p, abi.c_dp]
+        L.cerb_resident_set_window_kind.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+        L.cerb_replay_configure_robot.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(abi.PreintConfig), C.c_int32, C.c_int32]
         self.cfg = cfg or abi.default_config()
         self.h = C.c_void_p()
         self._check(L.cerb_create(C.byref(self.cfg), C.byref(self.h)))
@@ -204,6 +209,17 @@ class Backend:
         self._check(self.lib.cerb_preintegrate_imu_batch(self.h, C.byref(pcfg), n, jobs, out.ctypes.data_as(C.POINTER(abi.IMUPreint))))
         return out
 
+    def preintegrate_mixed(self, cfgs, use_leg, jobs, n, cfg_of):
+        """cerb_preintegrate_mixed: job j under cfgs[cfg_of[j]]; returns (IMU-leg records [n], IMU records [n]), entry j filled in the array of
+        the kind use_leg[cfg_of[j]] names (the other array's entry j stays zero)."""
+        table = (abi.PreintConfig * len(cfgs))(*cfgs)
+        leg = np.ascontiguousarray(use_leg, dtype=np.int32); of = np.ascontiguousarray(cfg_of, dtype=np.int32)
+        out, out_imu = np.zeros(n, dtype=abi.preint_dtype), np.zeros(n, dtype=abi.imu_preint_dtype)
+        i32p = C.POINTER(C.c_int32)
+        self._check(self.lib.cerb_preintegrate_mixed(self.h, len(cfgs), table, leg.ctypes.data_as(i32p), n, jobs, of.ctypes.data_as(i32p),
+                                                     out.ctypes.data_as(C.POINTER(abi.IMULegPreint)), out_imu.ctypes.data_as(C.POINTER(abi.IMUPreint))))
+        return out, out_imu
+
     def eval_prior(self, prior, state, n_cols):
         res, jac = np.zeros(prior.n), np.zeros(prior.n * n_cols)
         self._check(self.lib.cerb_eval_prior(self.h, C.byref(prior), C.byref(state), _p(res), _p(jac)))
@@ -262,6 +278,21 @@ class Backend:
         sum_dt = np.zeros(n)
         self._check(self.lib.cerb_resident_preintegrate(self.h, C.byref(pcfg), n, jobs, windows.ctypes.data_as(C.POINTER(C.c_int32)), slots.ctypes.data_as(C.POINTER(C.c_int32)), _p(sum_dt)))
         return sum_dt
+
+    def resident_preintegrate_mixed(self, cfgs, jobs, n, cfg_of, windows, slots):
+        """resident_preintegrate with job j under cfgs[cfg_of[j]], the record kind that of window windows[j]; returns sum_dt [n]"""
+        table = (abi.PreintConfig * len(cfgs))(*cfgs)
+        i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
+        of, windows, slots = i32(cfg_of), i32(windows), i32(slots)
+        sum_dt = np.zeros(n)
+        i32p = C.POINTER(C.c_int32)
+        self._check(self.lib.cerb_resident_preintegrate_mixed(self.h, len(cfgs), table, n, jobs, of.ctypes.data_as(i32p), windows.ctypes.data_as(i32p),
+                                                              slots.ctypes.data_as(i32p), _p(sum_dt)))
+        return sum_dt
+
+    def resident_set_window_kind(self, w, use_leg):
+        """record kind of one empty resident window: IMU-leg records (use_leg) or IMU records"""
+        self._check(self.lib.cerb_resident_set_window_kind(self.h, w, 1 if use_leg else 0))
 
     def resident_upload(self, batch, pre_slots=None):
         """feature lists (obs_offset = slot * NUM_FRAMES), open flags and states of batch against the resident data; pre_slots [n, 10]"""

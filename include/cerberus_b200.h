@@ -341,6 +341,13 @@ int cerb_preintegrate_batch(CerbHandle *h, const CerbPreintConfig *cfg, int32_t 
 int cerb_preintegrate_imu_batch(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs,
                                 CerbIMUPreint *out);
 
+/* Jobs of several configurations in one launch: job j uses cfgs[cfg_of[j]] (0 <= cfg_of[j] < n_cfg); IMULegIntegrationBase into out[j]
+ * where use_leg[cfg_of[j]], IntegrationBase into out_imu[j] otherwise (the other array's entry j is not touched; an array no job writes
+ * may be NULL).  Each job's result is the one the single-configuration call above would give it.  cerb_preintegrate_batch and
+ * cerb_preintegrate_imu_batch are this call with a one-entry table. */
+int cerb_preintegrate_mixed(CerbHandle *h, int32_t n_cfg, const CerbPreintConfig *cfgs, const int32_t *use_leg, int32_t n,
+                            const CerbPreintJob *jobs, const int32_t *cfg_of, CerbIMULegPreint *out, CerbIMUPreint *out_imu);
+
 /* A1 leg kinematics (src/legKinematics/A1Kinematics.cpp:7-40), n legs:
  *   q [n][3], rho_opt [n] (lc), rho_fix [n][4];
  *   fk [n][3]; jac [n][9] column-major; dfk_drho [n][3]; dJ_dq [n][27] col-major 9x3; dJ_drho [n][9].
@@ -422,17 +429,25 @@ typedef struct CerbTrackEdit {         /* feature_per_frame.erase(begin() + posi
                                           (feature_manager.cpp:450-506), WINDOW_SIZE - 1 - start_frame for removeFront (:508-529) */
     int32_t window, slot, n_obs, position;         /* n_obs: observations the track holds before the edit */
 } CerbTrackEdit;
-/* Start n resident windows with empty stores, identity slot tables and no prior.  use_leg: 1 = CerbIMULegPreint records (USE_LEG == 1),
- * 0 = CerbIMUPreint records. */
+/* Start n resident windows with empty stores, identity slot tables and no prior.  use_leg: the record kind of every window, 1 =
+ * CerbIMULegPreint records (USE_LEG == 1), 0 = CerbIMUPreint records. */
 int cerb_resident_start(CerbHandle *h, int32_t n, int32_t use_leg);
+/* Change the record kind of one window (windows of both kinds may share a batch: a VINS window has no leg-bias block).  Accepted only on an
+ * empty window: no observation put since cerb_resident_start (or since the window's extent was reset) and no valid prior.  The window's
+ * preintegration slots are zeroed, so no record of the other kind survives. */
+int cerb_resident_set_window_kind(CerbHandle *h, int32_t window, int32_t use_leg);
 /* Scatter observations into the track stores / apply one erase per listed track (a track may be listed once per call). */
 int cerb_resident_put_observations(CerbHandle *h, int32_t count, const CerbTrackPut *puts);
 int cerb_resident_edit_tracks(CerbHandle *h, int32_t count, const CerbTrackEdit *edits);
-/* cerb_preintegrate_batch / cerb_preintegrate_imu_batch (by the use_leg of cerb_resident_start) with the result of job j left in
+/* cerb_preintegrate_batch / cerb_preintegrate_imu_batch (by the record kind of window windows[j]) with the result of job j left in
  * preintegration slot slots[j] of window windows[j], in the layout an upload of the record would have produced; only sum_dt (optional,
  * [n]) returns to the host.  slideWindowNew's merge of two intervals (estimator.cpp:1576-1616) is one job over both sample buffers. */
 int cerb_resident_preintegrate(CerbHandle *h, const CerbPreintConfig *cfg, int32_t n, const CerbPreintJob *jobs, const int32_t *windows,
                                const int32_t *slots, double *sum_dt);
+/* cerb_resident_preintegrate with job j under cfgs[cfg_of[j]] (0 <= cfg_of[j] < n_cfg): one launch for jobs of several configurations; the
+ * record kind is that of window windows[j].  cerb_resident_preintegrate is this call with a one-entry table. */
+int cerb_resident_preintegrate_mixed(CerbHandle *h, int32_t n_cfg, const CerbPreintConfig *cfgs, int32_t n, const CerbPreintJob *jobs,
+                                     const int32_t *cfg_of, const int32_t *windows, const int32_t *slots, double *sum_dt);
 /* cerb_batch_upload against the resident data: of descs[w] only n_features, features (obs_offset = slot * CERB_NUM_FRAMES), extrinsic_open
  * and td_open are read; states as in cerb_batch_upload; pre_slots [n][CERB_WINDOW_SIZE]: slot of interval i -> i + 1, a permutation of
  * 0 .. CERB_WINDOW_SIZE - 1 per window.  n must be the n of cerb_resident_start.  Afterwards the resident batch is used as after
@@ -451,8 +466,8 @@ int cerb_resident_marginalize(CerbHandle *h, const int32_t *flags, const CerbWin
 /* Seed or replace the prior of one window from the host (prior->valid == 0 removes it). */
 int cerb_resident_set_prior(CerbHandle *h, int32_t window, const CerbPrior *prior);
 /* Read one window's store back as ordinary CerbWindowDesc content (tests, debugging): obs [max_obs] slot by slot; preint or imu_preint
- * [CERB_WINDOW_SIZE] by preintegration slot, the members an upload carries filled in and the others zero (pass the one that matches use_leg,
- * NULL for the other); prior with linearized_jacobians / linearized_residuals pointing at storage for CERB_MAX_PRIOR_DIM^2 / CERB_MAX_PRIOR_DIM
+ * [CERB_WINDOW_SIZE] by preintegration slot, the members an upload carries filled in and the others zero (pass the one that matches the
+ * window's record kind, NULL for the other); prior with linearized_jacobians / linearized_residuals pointing at storage for CERB_MAX_PRIOR_DIM^2 / CERB_MAX_PRIOR_DIM
  * doubles.  Any output may be NULL. */
 int cerb_resident_read_window(CerbHandle *h, int32_t window, CerbObservation *obs, CerbIMULegPreint *preint, CerbIMUPreint *imu_preint,
                               CerbPrior *prior);
@@ -477,10 +492,21 @@ typedef struct CerbImage {
     const uint8_t *has1;       /* [n] */
     const double *pts1;        /* [n][7] */
 } CerbImage;
-/* h must have max_batch >= n_robots and max_features >= 2 * max_features of the replay (the triangulation batch holds every track). */
+/* h must have max_batch >= n_robots and max_features >= 2 * max_features of the replay (the triangulation batch holds every track).
+ * pcfg, estimate_extrinsic and estimate_td are every robot's configuration until cerb_replay_configure_robot changes it; every robot starts
+ * with use_leg = 1. */
 int cerb_replay_create(CerbHandle *h, const CerbPreintConfig *pcfg, int32_t n_robots, int32_t max_features, int32_t estimate_extrinsic,
                        int32_t estimate_td, CerbReplay **out);
 void cerb_replay_destroy(CerbReplay *r);
+/* The configuration of one robot, as setParameter() would load it from its yaml: use_leg = USE_LEG (0: processIMU, IntegrationBase,
+ * IMUFactor, no leg-bias blocks, estimator.cpp:554-588, :1160-1171; slideWindow's USE_IMU-only branches move no Rho and double2vector
+ * leaves Rho alone, so the rho columns of its path rows keep their seeded value), pcfg = its noise / kinematics globals (a use_leg = 0 robot
+ * reads acc_n, gyr_n, acc_w, gyr_w only), estimate_extrinsic, estimate_td.  The leg fields (phi, dphi, c) of a use_leg = 0 robot's
+ * CerbIMULegSamples are ignored.  Robots of both kinds step together, their intervals in one preintegration launch.  The robot must not be
+ * seeded (just created, or reset); cerb_replay_reset_robot keeps the configuration.  Works before or after cerb_replay_set_resident.  A
+ * rejected call changes nothing. */
+int cerb_replay_configure_robot(CerbReplay *r, int32_t robot, int32_t use_leg, const CerbPreintConfig *pcfg, int32_t estimate_extrinsic,
+                                int32_t estimate_td);
 int cerb_replay_set_extrinsics(CerbReplay *r, int32_t robot, const double *tic /* [2][3] */, const double *ric /* [2][9] row-major */);
 /* Seed frame k = 0 .. WINDOW_SIZE of a robot: states P, R (row-major), V; `first` = the IMU / leg sample at the previous frame instant (at
  * frame 0: at frame 0), `samples` = the interval k-1 -> k (ignored for k = 0); image = the tracked features of frame k (NULL for k = WINDOW_SIZE:
@@ -520,7 +546,7 @@ int cerb_replay_traffic(CerbReplay *r, int64_t *h2d_bytes, int64_t *d2h_bytes, i
 /* The window of one robot as the replay would upload it for a per-feature step (every track, in list order), for tests and debugging.
  * desc points into the replay's own arrays (valid until the next call on r): in the default mode tracks, observations, the preintegration
  * records and the prior; in resident mode the tracks only (obs_offset = slot * CERB_NUM_FRAMES) and prior.valid.  ids [<= max_ids] feature
- * ids; preint_current [CERB_WINDOW_SIZE]: 1 where the record of interval i -> i + 1 is up to date (0: samples were added since);
+ * ids; the records are desc->imu_preint (desc->preint NULL) for a use_leg = 0 robot; preint_current [CERB_WINDOW_SIZE]: 1 where the record of interval i -> i + 1 is up to date (0: samples were added since);
  * pre_slots [CERB_WINDOW_SIZE]: resident mode's slot of that interval. */
 int cerb_replay_window(CerbReplay *r, int32_t robot, CerbWindowDesc *desc, int32_t *ids, int32_t max_ids, int32_t *preint_current,
                        int32_t *pre_slots);
