@@ -834,6 +834,24 @@ CERB_D double ambient_sq(const double *a, const double *b, const double *la, con
     return t;
 }
 
+// t +/- w_f . v for the column w_f = W[0..NX)[f] of the L2-resident W (pointer to W[0][f], row stride F), accumulated in row order.  The loads
+// of a batch of rows are all issued before its first FMA: written as one loop, the body was compiled as load, FMA, load, ... (the next load
+// re-used the register of the FMA operand), one L2 round trip per row -- 79 in a row for every feature.
+template <bool SUB>
+CERB_D double w_column_dot(const double *wf, int F, const double *v, double t) {
+    constexpr int BATCH = 16;
+    for (int a0 = 0; a0 < NX; a0 += BATCH) {
+        double wr[BATCH];
+        _Pragma("unroll")
+        for (int u = 0; u < BATCH; u++) wr[u] = (a0 + u < NX) ? wf[(size_t)(a0 + u) * F] : 0.0;
+        _Pragma("unroll")
+        for (int u = 0; u < BATCH; u++) {
+            if (a0 + u < NX) { if (SUB) t -= wr[u] * v[a0 + u]; else t += wr[u] * v[a0 + u]; }
+        }
+    }
+    return t;
+}
+
 // ---- S' = S - T T^T for one warp (see the call site).  The 55 upper 8 x 8 blocks of the 80 x 80 Gram matrix of [T; gy'^T] are dealt to
 // the 8 warps as rectangles of the block grid, so that a warp's 6-7 blocks share 4-7 fragment rows: 40 fragment loads per k-step
 // and CTA instead of 110 (the row stride of T, 143 doubles, makes every fragment load a 4-way bank conflict, and the loop was bound
@@ -1204,14 +1222,14 @@ CERB_D void ttt_warp_w(int wq, Smem &s, int lane) {
 // W' is staged through shared memory 32 features at a time as an 80-row tile whose row 78 carries
 // g_l / sqrt(h + mu D^2) (so that column 78 of the Gram matrix is the rhs update) and row 79 is zero.
 // The 55 upper 8x8 blocks of the 80x80 Gram matrix go to the 7 warps as row strips (SCPlan, compile-time).
-CERB_D void lambda_schur(Smem &s, const Win &c, double mu, int tid PH_ARG) {
-    const int F = c.ws.F, nF = c.nF;
-    const double *W = c.ws.W, *hh = c.ws.hh, *gl = c.ws.gl, *Dl = c.ws.Dl, *stl = c.ws.stl;
+CERB_D void lambda_schur(Smem &s, const CtaWs &ws, int nF, double mu, int tid PH_ARG) {
+    const int F = ws.F;
+    const double *W = ws.W, *hh = ws.hh, *gl = ws.gl, *Dl = ws.Dl, *stl = ws.stl;
     const int t2 = tid - 32, n2 = SOLVE_THREADS - 32;
     const int wq = (tid >> 5) - 1, lane = tid & 31;
     const int LDW = SC_LDW;
     double *tw = s.Ju;                         // 80 x 36 tile (aliases Ju .. red, unused during the solve)
-    double *sinv = nF <= 1024 ? s.wj : c.ws.sinv;  // 1 / sqrt(h + mu D^2): shared memory (wj: 1024 doubles) up to the reference's NUM_OF_F,
+    double *sinv = nF <= 1024 ? s.wj : ws.sinv;  // 1 / sqrt(h + mu D^2): shared memory (wj: 1024 doubles) up to the reference's NUM_OF_F,
                                                    // the ninth workspace vector for the larger synthetic stress windows
     {   // Cauchy point (H still unregularised / unfactored here)
         const double *v = s.stp;
@@ -1219,8 +1237,7 @@ CERB_D void lambda_schur(Smem &s, const Win &c, double mu, int tid PH_ARG) {
         for (int k = t2; k < NX * NX; k += n2) pv += v[k / NX] * s.Hxx[k] * v[k % NX];
         for (int k = t2; k < NX * NY; k += n2) pv += 2.0 * v[k / NY] * s.Hxy[k] * v[NX + k % NY];
         for (int f = t2; f < nF; f += n2) {
-            double wv = 0.0;
-            for (int a = 0; a < NX; a++) wv += W[(size_t)a * F + f] * v[a];
+            const double wv = w_column_dot<false>(W + f, F, v, 0.0);
             pv += 2.0 * stl[f] * wv + hh[f] * stl[f] * stl[f];
         }
         for (int o = 16; o > 0; o >>= 1) pv += __shfl_sync(0xffffffffu, pv, (lane + o) & 31);
@@ -1391,8 +1408,33 @@ CERB_D void panel_cholesky(Smem &s, int tid) {
         __syncthreads();
     }
 }
+// The three parts of the Gauss-Newton step below are real calls, like vision_linearize: each gets its own register allocation.  Inlined
+// into the kernel body (at the 255-register cap with spills) the per-feature loops over W were scheduled as load, FMA, load, ...
+// Hyy chain factorisation (warp 0) | Cauchy point, inverse-depth Schur complement and forward substitution (warps 1..7)
+CERB_NOINLINE void gn_eliminate(const SolveParams &P, int w, double mu, int tid PH_ARG) {
+    CERB_DYN_SMEM(double, smem_base);
+    Smem s; smem_carve(smem_base, s);
+    int *chain_done = s.ti + TI_CHAIN_DONE;
+    if (tid < 32) chain_cholesky(s, chain_done, tid PH_FWD);
+    else { lambda_schur(s, ws_carve(P), P.n_features[w], mu, tid PH_FWD); forward_subst(s, chain_done, tid - 32); }
+}
+// S' = S - T T^T (lower), rhs'_x = rhs_x - T gy' : Gram matrix of the 79 x 143 matrix [T; gy'^T] on the fp64 tensor cores, K = 143
+// padded to 144, block rectangles per warp (ttt_warp); then the dense Cholesky of S'
+CERB_NOINLINE void gn_reduce_factor(int tid PH_ARG) {
+    CERB_DYN_SMEM(double, smem_base);
+    Smem s; smem_carve(smem_base, s);
+    ttt_warp_w(tid >> 5, s, tid & 31);
+    __syncthreads();
+    PH_MARK(9);
+    panel_cholesky(s, tid);
+    PH_MARK(10);
+}
 // back substitutions for y_x, y_y and the inverse depths; the prior image's Hxx part is prefetched as soon as the factor of Hxx is dead
-CERB_D void back_substitution(const SolveParams &P, Smem &s, const Win &c, PriorCopy &pc, double mu, int &gn_attempts, int tid PH_ARG) {
+// (fail: report the solve as failed, the fault injection of the parity tests)
+CERB_NOINLINE void back_substitution(const SolveParams &P, int w, bool has_prior, bool bulk_ok, double mu, bool fail, int tid PH_ARG) {
+    CERB_DYN_SMEM(double, smem_base);
+    Smem s; smem_carve(smem_base, s);
+    const CtaWs ws = ws_carve(P);
     // L^T y_x = z by warp 0: lane holds y[lane], y[lane + 32], y[lane + 64] in registers;
     // branch-free steps (selects), the L entries of the next step are loaded before the current shuffle completes
     if (tid < 32) {
@@ -1411,10 +1453,9 @@ CERB_D void back_substitution(const SolveParams &P, Smem &s, const Win &c, Prior
         s.yv[tid] = y0; s.yv[32 + tid] = y1; if (64 + tid < NX) s.yv[64 + tid] = y2;
     }
     __syncthreads();
-    if (c.has_prior) {                                                                         // the factor of Hxx is dead from here on
-        if (c.bulk_ok) { if (tid == 0) CERB_BULK_G2S(s.Hxx, c.ws.pimg, PIMG_HXY * 8, &s.mbar[0]); }
-        else copy_g2s_async(s.Hxx, c.ws.pimg, HXX_SZ, tid);
-        pc.hxx_prefetched = true;
+    if (has_prior) {                                                                           // the factor of Hxx is dead from here on
+        if (bulk_ok) { if (tid == 0) CERB_BULK_G2S(s.Hxx, ws.pimg, PIMG_HXY * 8, &s.mbar[0]); }
+        else copy_g2s_async(s.Hxx, ws.pimg, HXX_SZ, tid);
     }
     PH_MARK(11);
     // y part: u = gy' - T^T y_x, then L^T y_y = u blockwise (warp 0)
@@ -1452,17 +1493,16 @@ CERB_D void back_substitution(const SolveParams &P, Smem &s, const Win &c, Prior
     PH_MARK(12);
     // inverse depths: y_l = (gl - w^T y_x) / (h + mu D^2) ; validity
     double bad = 0.0;
-    for (int f = tid; f < c.nF; f += SOLVE_THREADS) {
-        double t = c.ws.gl[f];
-        for (int a = 0; a < NX; a++) t -= c.ws.W[(size_t)a * c.ws.F + f] * s.yv[a];
-        const double y = t / (c.ws.hh[f] + mu * c.ws.Dl[f] * c.ws.Dl[f]);
-        c.ws.gnl[f] = y;
+    const int nF = P.n_features[w];
+    for (int f = tid; f < nF; f += SOLVE_THREADS) {
+        const double t = w_column_dot<true>(ws.W + f, ws.F, s.yv, ws.gl[f]);
+        const double y = t / (ws.hh[f] + mu * ws.Dl[f] * ws.Dl[f]);
+        ws.gnl[f] = y;
         if (!(fabs(y) < 1e300)) bad = 1.0;
     }
     for (int k = tid; k < NR; k += SOLVE_THREADS) if (!(fabs(s.yv[k]) < 1e300)) bad = 1.0;
     if (bad != 0.0) s.sca[S_OK] = 0;          // benign race: every writer stores 0
-    if (gn_attempts < P.test_fail_factorizations) s.sca[S_OK] = 0;      // fault injection of the parity tests (0 in production)
-    gn_attempts++;
+    if (fail) s.sca[S_OK] = 0;
     __syncthreads();
     PH_MARK(13);
 }
@@ -1475,11 +1515,9 @@ CERB_D void gauss_newton_step(const SolveParams &P, Smem &s, const Win &c, Prior
         s.yv[k] = s.g[k];
         if (k >= NX) s.Ad[((k - NX) / NYB) * HBLK + ((k - NX) % NYB) * (NYB + 1)] += mu * s.D[k] * s.D[k];
     }
-    int *chain_done = s.ti + TI_CHAIN_DONE;
-    if (tid == 0) *chain_done = 0;
+    if (tid == 0) s.ti[TI_CHAIN_DONE] = 0;
     __syncthreads();
-    if (tid < 32) chain_cholesky(s, chain_done, tid PH_FWD);
-    else { lambda_schur(s, c, mu, tid PH_FWD); forward_subst(s, chain_done, tid - 32); }
+    gn_eliminate(P, c.w, mu, tid PH_FWD);
     __syncthreads();
     if (tid == 0) {
         double vhv = s.sca[S_VHV];
@@ -1489,14 +1527,10 @@ CERB_D void gauss_newton_step(const SolveParams &P, Smem &s, const Win &c, Prior
     PH_MARK(5);
     __syncthreads();
     PH_MARK(8);
-    // S' = S - T T^T (lower), rhs'_x = rhs_x - T gy' : Gram matrix of the 79 x 143 matrix [T; gy'^T] on the
-    // fp64 tensor cores, K = 143 padded to 144; block rectangles per warp, see ttt_warp
-    ttt_warp_w(tid >> 5, s, tid & 31);
-    __syncthreads();
-    PH_MARK(9);
-    panel_cholesky(s, tid);
-    PH_MARK(10);
-    back_substitution(P, s, c, pc, mu, gn_attempts, tid PH_FWD);
+    gn_reduce_factor(tid PH_FWD);
+    back_substitution(P, c.w, c.has_prior, c.bulk_ok, mu, gn_attempts < P.test_fail_factorizations, tid PH_FWD);
+    if (c.has_prior) pc.hxx_prefetched = true;
+    gn_attempts++;
     if (s.sca[S_OK] != 0.0) {      // gauss_newton_step = -D * y ; norms for the dogleg
         double part3[2] = {0.0, 0.0};    // ||gn||^2, gh . gn
         for (int k = tid; k < NR; k += SOLVE_THREADS) { const double v = -s.D[k] * s.yv[k]; s.gn[k] = v; part3[0] += v * v; part3[1] += s.gh[k] * v; }

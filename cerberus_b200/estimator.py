@@ -569,7 +569,12 @@ class NativeReplay:
 
     def close(self):
         if self.r:
-            self.be.lib.cerb_replay_destroy(self.r); self.r = C.c_void_p()
+            # cerb_replay_destroy unregisters the replay's host buffers from its handle.  When the replay and its Backend are garbage of
+            # one reference cycle, their finalizers run in any order: if the handle is already destroyed, the replay's host object is
+            # left to the process exit instead of being freed through a dangling handle.
+            if self.be.h:
+                self.be.lib.cerb_replay_destroy(self.r)
+            self.r = C.c_void_p()
 
     def __del__(self):
         try: self.close()
