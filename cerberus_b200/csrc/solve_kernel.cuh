@@ -1320,7 +1320,7 @@ CERB_D void forward_subst(Smem &s, const int *chain_done, int t2) {
 // block by block on the fp64 tensor cores (A_ij -= L_ik L_jk^T, K = 8) -- warp 0 takes only the block that becomes
 // the next diagonal block and factors it right away, while warps 1..7 update the rest.  Two barriers per panel; the
 // serial column sweeps of the diagonal blocks (the critical path) overlap with the trailing updates.
-CERB_D void panel_cholesky(Smem &s, int tid) {
+CERB_D void panel_cholesky(Smem &s, int tid PH_ARG) {
     const int wq = tid >> 5, lane = tid & 31;
     auto factor_diag = [&](int c0, int nb, double *Lkk) {      // warp 0: L_kk of the nb x nb block at (c0, c0); Lkk[64..72) = 1 / diag
         const bool act = lane < nb;
@@ -1392,6 +1392,7 @@ CERB_D void panel_cholesky(Smem &s, int tid) {
             for (int c = 0; c < 8; c++) if (c < nb) row[c] = t[c];
         }
         __syncthreads();
+        PH_MARK(47);
         if (c1 >= NX) break;
         // (c) trailing update of rows / columns c1 .. NX (row NX = rhs) + look-ahead factorisation of the next diagonal block
         {
@@ -1401,11 +1402,14 @@ CERB_D void panel_cholesky(Smem &s, int tid) {
                 trailing_block(c0, b0, 0);
                 __syncwarp();
                 factor_diag(c1, (NX - c1) < 8 ? (NX - c1) : 8, s.red + 80 * (pk ^ 1));
+                PH_MARK(44);
             } else {
                 for (int b = wq; b < nblk; b += 7) trailing_block(c0, b0, b);
+                PH_MARK_T(45, 32);
             }
         }
         __syncthreads();
+        PH_MARK(46);
     }
 }
 // The three parts of the Gauss-Newton step below are real calls, like vision_linearize: each gets its own register allocation.  Inlined
@@ -1426,31 +1430,32 @@ CERB_NOINLINE void gn_reduce_factor(int tid PH_ARG) {
     ttt_warp_w(tid >> 5, s, tid & 31);
     __syncthreads();
     PH_MARK(9);
-    panel_cholesky(s, tid);
+    panel_cholesky(s, tid PH_FWD);
     PH_MARK(10);
 }
 // back substitutions for y_x, y_y and the inverse depths; the prior image's Hxx part is prefetched as soon as the factor of Hxx is dead
-// (fail: report the solve as failed, the fault injection of the parity tests)
+// (fail: report the solve as failed, the fault injection of the parity tests).  The inverse depths need only y_x: warps 5..7 start them
+// as soon as y_x is solved, warps 1..4 join after their share of T^T y_x, while warp 0 runs the y substitution.
 CERB_NOINLINE void back_substitution(const SolveParams &P, int w, bool has_prior, bool bulk_ok, double mu, bool fail, int tid PH_ARG) {
     CERB_DYN_SMEM(double, smem_base);
     Smem s; smem_carve(smem_base, s);
     const CtaWs ws = ws_carve(P);
-    // L^T y_x = z by warp 0: lane holds y[lane], y[lane + 32], y[lane + 64] in registers;
-    // branch-free steps (selects), the L entries of the next step are loaded before the current shuffle completes
-    if (tid < 32) {
-        double y0 = s.yv[tid], y1 = s.yv[32 + tid], y2 = (64 + tid < NX) ? s.yv[64 + tid] : 0.0;
+    const int wq = tid >> 5, lane = tid & 31;
+    if (wq == 0) {      // L^T y_x = z: lane holds y[lane], y[lane + 32], y[lane + 64] in registers; branch-free steps (selects), the L entries
+                        // of the next step are loaded before the current shuffle completes
+        double y0 = s.yv[lane], y1 = s.yv[32 + lane], y2 = (64 + lane < NX) ? s.yv[64 + lane] : 0.0;
         _Pragma("unroll 1")
         for (int k = NX - 1; k >= 0; k--) {
             const double *Lk = s.Hxx + k * NX;
             const double ik = s.idx[k];
-            const double l0 = (tid < k) ? Lk[tid] : 0.0, l1 = (32 + tid < k) ? Lk[32 + tid] : 0.0, l2 = (64 + tid < k) ? Lk[64 + tid] : 0.0;
+            const double l0 = (lane < k) ? Lk[lane] : 0.0, l1 = (32 + lane < k) ? Lk[32 + lane] : 0.0, l2 = (64 + lane < k) ? Lk[64 + lane] : 0.0;
             const double src = (k >= 64) ? y2 : (k >= 32 ? y1 : y0);
             const double yk = __shfl_sync(0xffffffffu, src, k & 31) * ik;
-            y0 = (tid == k) ? yk : y0 - l0 * yk;
-            y1 = (32 + tid == k) ? yk : y1 - l1 * yk;
-            y2 = (64 + tid == k) ? yk : y2 - l2 * yk;
+            y0 = (lane == k) ? yk : y0 - l0 * yk;
+            y1 = (32 + lane == k) ? yk : y1 - l1 * yk;
+            y2 = (64 + lane == k) ? yk : y2 - l2 * yk;
         }
-        s.yv[tid] = y0; s.yv[32 + tid] = y1; if (64 + tid < NX) s.yv[64 + tid] = y2;
+        s.yv[lane] = y0; s.yv[32 + lane] = y1; if (64 + lane < NX) s.yv[64 + lane] = y2;
     }
     __syncthreads();
     if (has_prior) {                                                                           // the factor of Hxx is dead from here on
@@ -1458,11 +1463,13 @@ CERB_NOINLINE void back_substitution(const SolveParams &P, int w, bool has_prior
         else copy_g2s_async(s.Hxx, ws.pimg, HXX_SZ, tid);
     }
     PH_MARK(11);
-    // y part: u = gy' - T^T y_x, then L^T y_y = u blockwise (warp 0)
-    for (int q = tid; q < NY; q += SOLVE_THREADS) { double t = 0.0; for (int a = 0; a < NX; a++) t += s.Hxy[a * NY + q] * s.yv[a]; s.yv[NX + q] -= t; }
-    __syncthreads();
-    if (tid < 32) {      // lane r holds component r of the current block; one shuffle per substitution step
-        const int r = tid < NYB ? tid : 0;
+    double bad = 0.0;
+    if (wq < 5) {       // y part: u = gy' - T^T y_x (threads 0..142), then L^T y_y = u blockwise (warp 0)
+        if (tid < NY) { double t = 0.0; for (int a = 0; a < NX; a++) t += s.Hxy[a * NY + tid] * s.yv[a]; s.yv[NX + tid] -= t; }
+        CERB_BAR_SYNC(1, 160);
+    }
+    if (wq == 0) {      // lane r holds component r of the current block; one shuffle per substitution step
+        const int r = lane < NYB ? lane : 0;
         double yn[NYB];                                  // solved block f + 1 (all lanes)
         _Pragma("unroll")
         for (int k = 0; k < NYB; k++) yn[k] = 0.0;
@@ -1479,28 +1486,28 @@ CERB_NOINLINE void back_substitution(const SolveParams &P, int w, bool has_prior
             }
             double lc[NYB], ig[NYB];                          // column r of L^T and the inverse pivots: loaded before the chain
             _Pragma("unroll")
-            for (int k = 0; k < NYB; k++) { lc[k] = (tid < k) ? L[k * NYB + r] : 0.0; ig[k] = s.idg[NYB * f + k]; }
+            for (int k = 0; k < NYB; k++) { lc[k] = (lane < k) ? L[k * NYB + r] : 0.0; ig[k] = s.idg[NYB * f + k]; }
             _Pragma("unroll")
             for (int k = NYB - 1; k >= 0; k--) {
                 const double yk = __shfl_sync(0xffffffffu, u, k) * ig[k];
                 yn[k] = yk;
-                u = (tid == k) ? yk : u - lc[k] * yk;
+                u = (lane == k) ? yk : u - lc[k] * yk;
             }
-            if (tid < NYB) s.yv[NX + NYB * f + tid] = u;
+            if (lane < NYB) s.yv[NX + NYB * f + lane] = u;
         }
+        __syncwarp();
+        for (int k = lane; k < NR; k += 32) if (!(fabs(s.yv[k]) < 1e300)) bad = 1.0;
+        PH_MARK(12);
+    } else {            // warps 1..7: inverse depths y_l = (gl - w^T y_x) / (h + mu D^2)
+        const int nF = P.n_features[w];
+        for (int f = tid - 32; f < nF; f += SOLVE_THREADS - 32) {
+            const double t = w_column_dot<true>(ws.W + f, ws.F, s.yv, ws.gl[f]);
+            const double y = t / (ws.hh[f] + mu * ws.Dl[f] * ws.Dl[f]);
+            ws.gnl[f] = y;
+            if (!(fabs(y) < 1e300)) bad = 1.0;
+        }
+        PH_MARK_T(43, 32);
     }
-    __syncthreads();
-    PH_MARK(12);
-    // inverse depths: y_l = (gl - w^T y_x) / (h + mu D^2) ; validity
-    double bad = 0.0;
-    const int nF = P.n_features[w];
-    for (int f = tid; f < nF; f += SOLVE_THREADS) {
-        const double t = w_column_dot<true>(ws.W + f, ws.F, s.yv, ws.gl[f]);
-        const double y = t / (ws.hh[f] + mu * ws.Dl[f] * ws.Dl[f]);
-        ws.gnl[f] = y;
-        if (!(fabs(y) < 1e300)) bad = 1.0;
-    }
-    for (int k = tid; k < NR; k += SOLVE_THREADS) if (!(fabs(s.yv[k]) < 1e300)) bad = 1.0;
     if (bad != 0.0) s.sca[S_OK] = 0;          // benign race: every writer stores 0
     if (fail) s.sca[S_OK] = 0;
     __syncthreads();

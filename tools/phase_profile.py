@@ -10,12 +10,15 @@ F = int(sys.argv[2]) if len(sys.argv) > 2 else 150
 REP = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 NAMES = {0: "zero+geometry", 1: "vision_linearize (total)", 2: "inertial_linearize (total)", 3: "post-linearize (sums, symmetrise, scaling)",
          4: "dogleg diag + Cauchy", 5: "Schur/Hyy join wait (warp0 after 6)", 6: "Hyy chain Cholesky (warp 0)", 7: "lambda Schur DMMA (warp 1)",
-         8: "T = L^-1 Hyx", 9: "S - T T^T DMMA", 10: "dense Cholesky 79", 11: "back-substitution x", 12: "y part", 13: "inverse depths",
+         8: "T = L^-1 Hyx", 9: "S - T T^T DMMA", 10: "dense Cholesky 79 (rest; panels in 44-47)", 11: "back-substitution x", 12: "y part (warp 0)", 13: "inverse depths (warp 0 waits)",
          14: "gn norms + dogleg scalars + step", 15: "apply_plus + geometry", 16: "vision_cost", 17: "inertial_cost + prior", 18: "accept / copy",
          20: "  vis: chunk setup", 21: "  vis: eval + tile write", 22: "  vis: DMMA Gram + partial store", 23: "  vis: reduce + scatter", 24: "  vis: per-feature tail",
          28: "    dmma loop (warp 0 view)", 29: "    partial stores + W (warp 0)", 30: "  imu: warps 0-2 (factor rounds, tail)", 32: "    imu warp 0: zero + expand Ju", 33: "    imu warp 0: whiten", 34: "    imu warp 0: S prefetch + Gram", 35: "    imu warp 0: scatter", 36: "    imu warp 0: round barrier", 31: "  imu: warps 3-7 (prior)",
          19: "  schur (warp 1): rhs + Cauchy v^T H v", 37: "  schur (warp 1): sinv + block table + first fetch", 38: "  schur (warp 1): tile scale/store + barrier (all tiles)", 39: "  schur (warp 1): DMMA loop + barrier (all tiles)",
-         25: "  imu: linearize (10 threads)", 26: "  imu: whiten + Gram x10", 27: "  imu: prior"}
+         25: "  imu: linearize (10 threads)", 26: "  imu: whiten + Gram x10", 27: "  imu: prior",
+         47: "  chol: first diag block + panel solve + barrier", 44: "  chol: warp 0 next diag block (update + factor)", 45: "  chol: trailing update (warp 1)",
+         46: "  chol: warp 0 wait at the panel barrier",
+         43: "  bsub: inverse depths (warp 1)"}
 cfg = abi.default_config(); cfg.max_batch = NW; cfg.max_features = 160; cfg.max_obs = 160 * 11
 gb = lib.Backend(cfg, lib_path=os.path.join(ROOT, "tools", "libcerberus_b200_prof.so"))
 batch = synth.generate_batch(min(NW, 8), F, gb, prior_features=24)
