@@ -566,6 +566,7 @@ class NativeReplay:
         if resident:
             backend._check(backend.lib.cerb_replay_set_resident(self.r, 1))
         self.reports = []
+        self._snap_cap = 1 << 19                      # save()'s first buffer, grown to the largest snapshot
 
     def close(self):
         if self.r:
@@ -617,6 +618,28 @@ class NativeReplay:
     def reset(self, robot):
         """The reference's estimator restart (clearState) for one robot; it is seeded again (seed_robot) before it steps."""
         self.be._check(self.be.lib.cerb_replay_reset_robot(self.r, robot))
+
+    def save(self, robot):
+        """cerb_replay_save_robot: a snapshot of a seeded robot (its state, prior and configuration, no path or flag history) as bytes.  It can
+        be loaded into any robot of any NativeReplay of this library build, in either mode and on any handle."""
+        L, size = self.be.lib, C.c_size_t()
+        while True:                                   # one call unless the snapshot outgrew the largest one so far
+            buf = C.create_string_buffer(self._snap_cap)
+            rc = L.cerb_replay_save_robot(self.r, robot, buf, self._snap_cap, C.byref(size))
+            if rc == 0: return buf.raw[:size.value]
+            if size.value <= self._snap_cap: self.be._check(rc)
+            self._snap_cap = size.value
+
+    def load(self, robot, blob):
+        """cerb_replay_load_robot: robot `robot` becomes the saved robot and continues as it would have; a rejected snapshot (CerbError)
+        changes nothing."""
+        blob = bytes(blob)
+        self.be._check(self.be.lib.cerb_replay_load_robot(self.r, robot, blob, len(blob)))
+
+    def clone(self, src, dsts):
+        """cerb_replay_clone_robot: robots `dsts` become copies of robot `src` (a save and a load each, in one batched call)."""
+        d = np.ascontiguousarray(dsts, dtype=np.int32)
+        self.be._check(self.be.lib.cerb_replay_clone_robot(self.r, src, len(d), d.ctypes.data_as(C.POINTER(C.c_int32))))
 
     def step(self, images, firsts, samples, header, robots=None, headers=None):
         """One camera frame of every robot at stamp `header`, or of the robots listed in `robots` (each at its own stamp headers[i] if given);

@@ -98,6 +98,9 @@ class Backend:
         L.cerb_resident_preintegrate_mixed.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.PreintConfig), C.c_int32, C.POINTER(abi.PreintJob), i32p, i32p, i32p, abi.c_dp]
         L.cerb_resident_set_window_kind.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
         L.cerb_replay_configure_robot.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(abi.PreintConfig), C.c_int32, C.c_int32]
+        L.cerb_replay_save_robot.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        L.cerb_replay_load_robot.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.c_size_t]
+        L.cerb_replay_clone_robot.argtypes = [C.c_void_p, C.c_int32, C.c_int32, i32p]
         self.cfg = cfg or abi.default_config()
         self.h = C.c_void_p()
         self._check(L.cerb_create(C.byref(self.cfg), C.byref(self.h)))

@@ -550,6 +550,27 @@ int cerb_replay_traffic(CerbReplay *r, int64_t *h2d_bytes, int64_t *d2h_bytes, i
  * pre_slots [CERB_WINDOW_SIZE]: resident mode's slot of that interval. */
 int cerb_replay_window(CerbReplay *r, int32_t robot, CerbWindowDesc *desc, int32_t *ids, int32_t max_ids, int32_t *preint_current,
                        int32_t *pre_slots);
+/* Snapshots of one robot: everything the robot carries that later steps read (its states, extrinsics, td, stamps, counters, the feature list
+ * in list order with every observation, the intervals with their samples and linearisation points, the marginalization prior and the robot's
+ * configuration), and nothing of where it lives on the device.  A robot saved after frame k and loaded into any robot of any replay, in
+ * either mode and on any handle, continues bit for bit as the saved robot does.  The path rows and the flag history are outputs and do not
+ * travel: a loaded robot starts both empty.  The buffer starts with a magic number, a format version, CERB_WINDOW_SIZE, the number of
+ * features and the prior dimension; it is meant for the same build of this library, not as a file format.
+ * save: the robot must be seeded.  *size = the snapshot's size in bytes; buf = NULL: nothing else, else the snapshot into buf [cap]
+ * (CERB_ERR_BAD_ARGUMENT if cap is smaller, *size still set: a caller can offer a buffer first and grow it once).  In resident mode the
+ * prior is read off the device. */
+int cerb_replay_save_robot(CerbReplay *r, int32_t robot, void *buf, size_t cap, size_t *size);
+/* Overwrite `robot` with a snapshot; it counts as seeded and is stepped as usual.  The snapshot is checked before anything changes (magic
+ * number, version, sizes against `size`, tracks against the replay's capacity: 2 x max_features tracks, max_features of them with four or
+ * more observations; observation counts against CERB_NUM_FRAMES, feature ids unique, the keyframe flag 0 or 1, the prior dimension against
+ * CERB_MAX_PRIOR_DIM and its blocks, no leg-bias block for a use_leg = 0 robot, the intervals against frame_count): a rejected snapshot returns CERB_ERR_BAD_ARGUMENT, moves nothing and leaves the robot as it was.  In
+ * resident mode the window is emptied and takes the snapshot's record kind, the observations are put into fresh track slots, the intervals
+ * whose records were up to date are preintegrated again (cerb_resident_preintegrate_mixed: the same bits) and the prior is set. */
+int cerb_replay_load_robot(CerbReplay *r, int32_t robot, const void *buf, size_t size);
+/* Make robots dsts[0 .. n - 1] of the same replay copies of robot src: one save and n loads, done in place.  Resident mode: one put stream
+ * and one preintegration launch for all of them, and the prior is copied from window to window on the device.  dsts must be distinct and not
+ * contain src; a rejected call changes nothing. */
+int cerb_replay_clone_robot(CerbReplay *r, int32_t src, int32_t n, const int32_t *dsts);
 
 /* ---- host-side helpers that stay on the CPU in the reference too ---------------------------- */
 /* Gauge re-anchoring of Estimator::double2vector (estimator.cpp:903-957): rotates the solved
